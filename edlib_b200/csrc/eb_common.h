@@ -283,6 +283,7 @@ struct SeedPlanParams {
     const int* thr;          // [numReads] threshold t per read (t < 0: read skipped), or nullptr: seed_threshold(m, kBound, Ls, seedK, -1)
     int kBound, seedK;
     int numReads;
+    int maxLen;              // no read of the launch is longer (0: unknown); bounds t and so the lanes a read needs
     int Ls;                  // seed length of this level
     int Lidx, sigma, numKeys;
     const int* bucketStart;

@@ -760,11 +760,12 @@ EB_HD void seed_fill_item(const SeedIndexParams& p, int i) {
     p.positions[p.bucketStart[b] + atomic_add_int(p.cursor + b, 1)] = i;
 }
 
-// Windows of one read from its sorted candidate end columns E[0..c): emit == false only counts them.
-// Windows start at multiples of 16 columns (a longer lead-in is still exact).  Candidates are verified together
-// as long as the window stays narrow enough for the banded sweep (k1b_sweep: tracked columns + 2t + 1 <= 64
-// diagonals); when t is too large for any banded window, as long as they are neighbours (gap / spread rule).
-EB_HD int seed_windows(const SeedPlanParams& p, const int* E, int c, int m, int t, int pair, int base, bool emit) {
+// Windows of one read from its sorted candidate end columns E[0..c): f(w, ws, lo, hi) for each window w in order;
+// returns their number.  Windows start at multiples of 16 columns (a longer lead-in is still exact).  Candidates are
+// verified together as long as the window stays narrow enough for the banded sweep (k1b_sweep: tracked columns +
+// 2t + 1 <= 64 diagonals); when t is too large for any banded window, as long as they are neighbours (gap / spread rule).
+template <class F>
+EB_HD int seed_windows(const SeedPlanParams& p, const int* E, int c, int m, int t, F&& f) {
     const int bandSlack = 63 - 4 * t;  // E[last] - E[first] may be this large in a banded window
     int prevHi = -1;
     int nW = 0;
@@ -788,22 +789,26 @@ EB_HD int seed_windows(const SeedPlanParams& p, const int* E, int c, int m, int 
         int ws = lo - (m + t);
         if (ws < 0) ws = 0;
         ws &= ~15;
-        if (emit) {
-            const int w = base + nW;
-            p.winPair[w] = pair;
-            p.winK[w] = t + 1;
-            p.winStart[w] = ws;
-            p.winLen[w] = hi - ws + 1;
-            p.winTf[w] = lo - ws;
-        }
+        f(nW, ws, lo, hi);
         ++nW;
     }
     return nW;
 }
+EB_HD void seed_window_store(const SeedPlanParams& p, int w, int pair, int t, int ws, int lo, int hi) {
+    p.winPair[w] = pair;
+    p.winK[w] = t + 1;
+    p.winStart[w] = ws;
+    p.winLen[w] = hi - ws + 1;
+    p.winTf[w] = lo - ws;
+}
 
-// Host spelling of the cooperative group that plans one read (one member); the device kernel passes a group of
-// eight lanes (four reads per warp).
+// Host spelling of the cooperative group that plans one read (one member); the device kernel passes groups of 16
+// or 32 lanes (eb_kernels.cu: CoopGroup).
+//   scan(v, total): exclusive prefix sum of v over the members, total = the sum over all of them;
+//   reserve(counter, n): every member of the group passes its read's n (all groups of a warp call it together on the
+//   device, which adds the warp's total to *counter once); returns the old value plus what the reads before it took.
 struct CoopSerial {
+    static constexpr int W = 1;
     static EB_HD int lane() { return 0; }
     static EB_HD int width() { return 1; }
     static EB_HD void sync() {}
@@ -813,151 +818,174 @@ struct CoopSerial {
         *p = old + v;
         return old;
     }
+    static EB_HD int scan(int v, int& total) {
+        total = v;
+        return 0;
+    }
+    static EB_HD int reserve(int* counter, int n) { return n > 0 ? atomic_add_int(counter, n) : 0; }
 };
 
-// Scratch of one planning group: E[CAP] candidate end columns, then SEED_CTL ints of control words:
-// ctl[0] candidates, ctl[1] saturated, ctl[2] long index ranges listed, ctl[3 + 3k ..] = {first, end, a} of range k.
-constexpr int SEED_LONG_RANGES = 16;
-constexpr int SEED_CTL = 3 + 3 * SEED_LONG_RANGES;
+// Scratch of one planning group of W members: E[CAP] candidate end columns, then seed_ctl_words(W) ints of control
+// words: ctl[0] candidates, ctl[1] saturated, then per member of the current round of seeds the first index entry
+// of its seed's range, the range's offset in the round's entries, and the seed's offset a in the read.
+EB_HD constexpr int seed_ctl_words(int W) { return 2 + 3 * W; }
+// enough control words for a group of any width (at most a warp); the device kernel reserves seed_ctl_words(W)
+constexpr int SEED_CTL = seed_ctl_words(32);
 
-// One occurrence list entry of seed read[a, a+Ls): verified against the target, its expected end column recorded.
-template <int CAP, class C>
-EB_HD void seed_try(const SeedPlanParams& p, const uint8_t* q, int m, int a, int Lk, int pos, int* E, int* ctl) {
-    bool same = pos + p.Ls <= p.n;  // keys near the end of the target were padded with code 0
-    for (int x = Lk; same && x < p.Ls; ++x) same = p.tcodes[pos + x] == q[a + x];
-    if (!same) return;
-    const int at = C::add_shared(&ctl[0], 1);
-    if (at < CAP) E[at] = pos + (m - a) - 1;
+// Candidates of one occurrence-list entry per slot k (pos < 0: none): the whole seed read[a, a+Ls) is compared with
+// the target (the key covered only its first Lk symbols) and the expected end column of each match recorded.
+// The loads of all slots are issued before any is used, so their latencies overlap.
+template <int CAP, int K, class C>
+EB_HD void seed_try(const SeedPlanParams& p, const uint8_t* q, int m, int Lk, const int (&pos)[K], const int (&a)[K],
+                    int* E, int* ctl) {
+    bool same[K];
+    EB_UNROLL
+    for (int k = 0; k < K; ++k) {
+        same[k] = pos[k] >= 0 && pos[k] + p.Ls <= p.n;  // keys near the end of the target were padded with code 0
+        if (same[k]) {
+            uint32_t diff = 0;
+            for (int x = Lk; x < p.Ls; ++x) diff |= (uint32_t)(p.tcodes[pos[k] + x] ^ q[a[k] + x]);
+            same[k] = diff == 0;
+        }
+    }
+    EB_UNROLL
+    for (int k = 0; k < K; ++k) {
+        if (!same[k]) continue;
+        const int at = C::add_shared(&ctl[0], 1);
+        if (at < CAP) E[at] = pos[k] + (m - a[k]) - 1;
+    }
 }
 
-// One read, planned by a cooperative group C (a single member on the host, eight lanes on the device).  The members
-// take the seeds of the read, so that the chains of dependent random reads (key -> index range -> positions -> target
-// symbols) of different seeds are in flight together; index ranges longer than a few entries per member (repeats,
-// short seeds) are set aside and then walked by the whole group together, a member's loads two at a time.  The
-// candidates meet in E; small sets are sorted by one member, larger ones by a bitonic network over the group.
+// One read, planned by a cooperative group C (a single member on the host, 16 or 32 lanes on the device).  Each
+// member takes one seed of the read, so that with as many members as seeds the key -> index range lookups of all
+// of them are in flight together.  The index entries of the round's ranges are then dealt out over the members as
+// one list (a member's entries loaded together: entry -> position -> target symbols), so a read with a long range
+// costs little more than one without.  The candidates meet in E and are sorted by a bitonic network over the
+// group; every member walks the sorted list to the same windows (seed_windows), keeps the one numbered like it and
+// writes it, and the group's reads of a warp take their room in the job arrays with one atomic (C::reserve).
+// Every member of every group of a warp must reach C::reserve: slots past numReads pass through with nothing.
 template <int CAP, class C>
 EB_HD void seed_plan_read(const SeedPlanParams& p, int slot, int* E, int* ctl) {
-    const int lane = C::lane(), W = C::width();
-    const int pair = p.readList ? p.readList[slot] : p.firstPair + slot;
-    const int m = p.qlen[pair];
-    const int t = p.thr ? p.thr[slot] : seed_threshold(m, p.kBound, p.Ls, p.seedK, -1);
-    const uint8_t* q = p.qcodes + p.qoff[pair];
+    const int lane = C::lane();
+    constexpr int W = C::W;
+    int* rStart = ctl + 2;      // [W]
+    int* rPre = rStart + W;     // [W]
+    int* rA = rPre + W;         // [W]
+    const bool live = slot < p.numReads;
+    const int pair = !live ? 0 : (p.readList ? p.readList[slot] : p.firstPair + slot);
+    const int m = live ? p.qlen[pair] : 0;
+    const int t = !live ? -1 : (p.thr ? p.thr[slot] : seed_threshold(m, p.kBound, p.Ls, p.seedK, -1));
+    const uint8_t* q = live ? p.qcodes + p.qoff[pair] : nullptr;
     SeedPlan pl;
     pl.first = pl.count = 0;
-    pl.state = SEED_NONE;
-    pl.thr = t;
-    if (t < 0) {  // left out of the stage (the host, or the threshold rule)
-        pl.state = SEED_SATURATED;
-        pl.thr = -1;
-        if (lane == 0) p.plan[slot] = pl;
-        return;
-    }
-    if (lane == 0) {
-        ctl[0] = 0;
-        ctl[1] = 0;
-        ctl[2] = 0;
-    }
-    C::sync();
-    const int stride = m / (t + 1);  // >= Ls: the t+1 pieces are disjoint
-    const int Lk = p.Ls < p.Lidx ? p.Ls : p.Lidx;  // symbols of the seed that go into the key
-    uint32_t span = 1;                             // keys sharing that prefix
-    for (int x = Lk; x < p.Lidx; ++x) span *= (uint32_t)p.sigma;
-    const int longFrom = 4;  // entries a member walks alone
-    for (int j0 = 0; j0 <= t; j0 += W) {
-        const int j = j0 + lane;
-        const int a = j * stride;
-        int i0 = 0, i1 = 0;
-        if (j <= t) {
-            // a code outside the target's alphabet (streamed batches give the reads' foreign bytes one) occurs nowhere
-            uint32_t key = 0;
-            bool known = true;
-            for (int x = 0; x < p.Ls; ++x) {
-                const uint32_t code = q[a + x];
-                known = known && code < (uint32_t)p.sigma;
-                if (x < Lk) key = key * (uint32_t)p.sigma + code;
-            }
-            if (known) {
-                key *= span;
-                i0 = p.bucketStart[key];
-                i1 = p.bucketStart[key + span];
-                if (i1 - i0 > p.maxBucket) {  // repeat: the read is passed on unseen
-                    ctl[1] = 1;
-                    i1 = i0;
-                } else if (i1 - i0 > longFrom) {
-                    const int k = C::add_shared(&ctl[2], 1);
-                    if (k < SEED_LONG_RANGES) {
-                        ctl[3 + 3 * k] = i0;
-                        ctl[4 + 3 * k] = i1;
-                        ctl[5 + 3 * k] = a;
-                        i1 = i0;  // walked by the whole group below
-                    }
-                }
-            }
-        }
-        for (int i = i0; i < i1; ++i) seed_try<CAP, C>(p, q, m, a, Lk, p.positions[i], E, ctl);
-    }
-    C::sync();
-    {
-        const int nLong = ctl[2] < SEED_LONG_RANGES ? ctl[2] : SEED_LONG_RANGES;
-        for (int k = 0; k < nLong; ++k) {
-            const int i1 = ctl[4 + 3 * k], a = ctl[5 + 3 * k];
-            int i = ctl[3 + 3 * k] + lane;
-            for (; i + W < i1; i += 2 * W) {  // two independent loads per round
-                const int pos0 = p.positions[i], pos1 = p.positions[i + W];
-                seed_try<CAP, C>(p, q, m, a, Lk, pos0, E, ctl);
-                seed_try<CAP, C>(p, q, m, a, Lk, pos1, E, ctl);
-            }
-            if (i < i1) seed_try<CAP, C>(p, q, m, a, Lk, p.positions[i], E, ctl);
-        }
-    }
-    C::sync();
-    const int c = ctl[0];
-    if (ctl[1] || c > CAP) {
+    pl.state = SEED_SATURATED;  // left out of the stage (the host, or the threshold rule) unless planned below
+    pl.thr = -1;
+    int c = 0;
+    if (t >= 0) {
+        pl.state = SEED_NONE;
+        pl.thr = t;
         if (lane == 0) {
-            pl.state = SEED_SATURATED;
-            p.plan[slot] = pl;
+            ctl[0] = 0;
+            ctl[1] = 0;
         }
-        return;
-    }
-    if (c > 32 && CAP >= 64) {
-        // bitonic network over the candidates padded to a power of two, compare-exchanges dealt to the members
-        int P2 = 64;
-        while (P2 < c) P2 *= 2;  // <= CAP (a power of two)
-        for (int i = c + lane; i < P2; i += W) E[i] = 0x7fffffff;
         C::sync();
-        for (int k = 2; k <= P2; k *= 2) {
-            for (int jj = k / 2; jj > 0; jj /= 2) {
-                for (int x = lane; x < P2 / 2; x += W) {
-                    const int lo = 2 * x - (x & (jj - 1));  // index with bit jj clear
-                    const int hi = lo + jj;
-                    const bool up = (lo & k) == 0;
-                    const int u = E[lo], v = E[hi];
-                    if ((u > v) == up) {
-                        E[lo] = v;
-                        E[hi] = u;
+        const int stride = m / (t + 1);  // >= Ls: the t+1 pieces are disjoint
+        const int Lk = p.Ls < p.Lidx ? p.Ls : p.Lidx;  // symbols of the seed that go into the key
+        uint32_t span = 1;                             // keys sharing that prefix
+        for (int x = Lk; x < p.Lidx; ++x) span *= (uint32_t)p.sigma;
+        for (int j0 = 0; j0 <= t; j0 += W) {  // one round when the group has t+1 members or more
+            const int j = j0 + lane;
+            const int a = j * stride;
+            int i0 = 0, len = 0;
+            if (j <= t) {
+                // a code outside the target's alphabet (streamed batches give the reads' foreign bytes one) occurs nowhere
+                uint32_t key = 0;
+                bool known = true;
+                for (int x = 0; x < p.Ls; ++x) {
+                    const uint32_t code = q[a + x];
+                    known = known && code < (uint32_t)p.sigma;
+                    if (x < Lk) key = key * (uint32_t)p.sigma + code;
+                }
+                if (known) {
+                    key *= span;
+                    i0 = p.bucketStart[key];
+                    len = p.bucketStart[key + span] - i0;
+                    if (len > p.maxBucket) {  // repeat: the read is passed on unseen
+                        ctl[1] = 1;
+                        len = 0;
                     }
                 }
-                C::sync();
+            }
+            int total;
+            const int pre = C::scan(len, total);
+            rStart[lane] = i0;
+            rPre[lane] = pre;
+            rA[lane] = a;
+            C::sync();
+            constexpr int K = 4;  // entries per member in flight together
+            for (int e0 = 0; e0 < total; e0 += K * W) {
+                int pos[K], aa[K];
+                EB_UNROLL
+                for (int k = 0; k < K; ++k) {
+                    const int e = e0 + k * W + lane;
+                    pos[k] = -1;
+                    aa[k] = 0;
+                    if (e < total) {
+                        int s = 0;  // the seed whose range holds entry e: the last one starting at or before it
+                        for (int h = W / 2; h > 0; h /= 2)
+                            if (rPre[s + h] <= e) s += h;
+                        aa[k] = rA[s];
+                        pos[k] = p.positions[rStart[s] + (e - rPre[s])];
+                    }
+                }
+                seed_try<CAP, K, C>(p, q, m, Lk, pos, aa, E, ctl);
+            }
+            C::sync();  // the round's ranges are walked before the next round overwrites them
+        }
+        c = ctl[0];
+        if (ctl[1] || c > CAP) {
+            pl.state = SEED_SATURATED;
+            c = 0;
+        } else if (c > 1) {
+            // bitonic network over the candidates padded to a power of two (<= CAP), compare-exchanges dealt to the members
+            int P2 = 2;
+            while (P2 < c) P2 *= 2;
+            for (int i = c + lane; i < P2; i += W) E[i] = 0x7fffffff;
+            C::sync();
+            for (int k = 2; k <= P2; k *= 2) {
+                for (int jj = k / 2; jj > 0; jj /= 2) {
+                    for (int x = lane; x < P2 / 2; x += W) {
+                        const int lo = 2 * x - (x & (jj - 1));  // index with bit jj clear
+                        const int hi = lo + jj;
+                        const bool up = (lo & k) == 0;
+                        const int u = E[lo], v = E[hi];
+                        if ((u > v) == up) {
+                            E[lo] = v;
+                            E[hi] = u;
+                        }
+                    }
+                    C::sync();
+                }
             }
         }
     }
-    if (lane != 0) return;
-    if (!(c > 32 && CAP >= 64)) {  // insertion sort (the usual case: a handful of candidates)
-        for (int i = 1; i < c; ++i) {
-            const int v = E[i];
-            int k = i - 1;
-            while (k >= 0 && E[k] > v) {
-                E[k + 1] = E[k];
-                --k;
-            }
-            E[k + 1] = v;
+    // every member walks the sorted candidates to the same windows and keeps the one numbered like it
+    int myWs = 0, myLo = 0, myHi = 0;
+    const int nW = seed_windows(p, E, c, m, t, [&](int w, int ws, int lo, int hi) {
+        if (w == lane) {
+            myWs = ws;
+            myLo = lo;
+            myHi = hi;
         }
-    }
-    const int nW = seed_windows(p, E, c, m, t, pair, 0, false);
+    });
+    const int base = C::reserve(p.winCount, nW);
     if (nW > 0) {
-        const int base = atomic_add_int(p.winCount, nW);
         if (base + nW <= p.winCap) {
-            seed_windows(p, E, c, m, t, pair, base, true);
+            if (lane < nW) seed_window_store(p, base + lane, pair, t, myWs, myLo, myHi);
+            if (nW > W)  // more windows than members (many candidates): the rest in a second walk
+                seed_windows(p, E, c, m, t, [&](int w, int ws, int lo, int hi) {
+                    if (w >= W && w % W == lane) seed_window_store(p, base + w, pair, t, ws, lo, hi);
+                });
             pl.first = base;
             pl.count = nW;
             pl.state = SEED_WINDOWS;
@@ -965,7 +993,7 @@ EB_HD void seed_plan_read(const SeedPlanParams& p, int slot, int* E, int* ctl) {
             pl.state = SEED_SATURATED;  // the job arrays are full (host-driven stages repeat with the exact size)
         }
     }
-    p.plan[slot] = pl;
+    if (live && lane == 0) p.plan[slot] = pl;
 }
 
 EB_HD void win_reduce_read(const WinReduceParams& p, int slot) {

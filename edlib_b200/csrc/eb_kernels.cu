@@ -415,38 +415,58 @@ __global__ void seed_fill_kernel(const SeedIndexParams p) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < p.numPos) seed_fill_item(p, i);
 }
-// One read per group of EIGHT lanes (four reads per warp): the lanes take the seeds of the read, so their index
-// lookups (key -> bucket bounds -> positions -> target symbols, a chain of dependent random reads) are in flight
-// together; candidates meet in shared memory, lane 0 of the group sorts them and emits the windows.
-struct CoopGroup8 {
-    static constexpr int W = 8;
-    static EB_D int lane() { return (int)(threadIdx.x & 7u); }
-    static EB_D int width() { return 8; }
-    static EB_D unsigned mask() { return 0xffu << (threadIdx.x & 24u); }
+// One read per group of GW lanes (16: two reads per warp; 32: a warp per read).  The lanes take the seeds of the
+// read, so their index lookups (key -> bucket bounds -> positions -> target symbols, a chain of dependent random
+// reads) are in flight together; candidates meet in shared memory (eb_core.h: seed_plan_read).
+template <int GW>
+struct CoopGroup {
+    static constexpr int W = GW;
+    static EB_D int lane() { return (int)(threadIdx.x & (GW - 1)); }
+    static EB_D int width() { return GW; }
+    static EB_D unsigned mask() { return GW == 32 ? 0xffffffffu : ((1u << (GW & 31)) - 1u) << (threadIdx.x & 31u & ~(GW - 1u)); }
     static EB_D void sync() { __syncwarp(mask()); }
     static EB_D bool any(bool v) { return __ballot_sync(mask(), v) != 0u; }
     static EB_D int add_shared(int* p, int v) { return atomicAdd(p, v); }
+    static EB_D int scan(int v, int& total) {
+        int incl = v;
+        EB_UNROLL
+        for (int d = 1; d < GW; d *= 2) {
+            const int y = __shfl_up_sync(mask(), incl, d, GW);
+            if (lane() >= d) incl += y;
+        }
+        total = __shfl_sync(mask(), incl, GW - 1, GW);
+        return incl - v;
+    }
+    // the whole warp: every lane holds its group's n, so a scan in steps of whole groups gives each lane the counts of
+    // its own and the earlier groups; one atomic for the warp's total, each group's offset in it
+    static EB_D int reserve(int* counter, int n) {
+        const int l32 = (int)(threadIdx.x & 31u);
+        int incl = n;
+        EB_UNROLL
+        for (int d = GW; d < 32; d *= 2) {
+            const int y = __shfl_up_sync(0xffffffffu, incl, d);
+            if (l32 >= d) incl += y;
+        }
+        const int total = __shfl_sync(0xffffffffu, incl, 31);
+        int base = 0;
+        if (total > 0) {
+            if (l32 == 31) base = atomicAdd(counter, total);
+            base = __shfl_sync(0xffffffffu, base, 31);
+        }
+        return base + incl - n;
+    }
 };
-// A whole warp per read: the last seed level sees few reads with long index ranges and thousands of candidates.
-struct CoopGroup32 {
-    static constexpr int W = 32;
-    static EB_D int lane() { return (int)(threadIdx.x & 31u); }
-    static EB_D int width() { return 32; }
-    static EB_D void sync() { __syncwarp(); }
-    static EB_D bool any(bool v) { return __any_sync(0xffffffffu, v) != 0; }
-    static EB_D int add_shared(int* p, int v) { return atomicAdd(p, v); }
-};
-// (CTAs of THREADS / 8 groups: the largest candidate capacity gets small CTAs so that its scratch fits shared memory)
+// (registers capped at 40 so that 48 warps fit an SM: the lookups of more reads are in flight together)
 template <int CAP, int THREADS, class Group>
-__global__ void __launch_bounds__(THREADS) seed_plan_kernel(const SeedPlanParams p) {
+__global__ void __launch_bounds__(THREADS, 1536 / THREADS) seed_plan_kernel(const SeedPlanParams p) {
     extern __shared__ __align__(16) unsigned char smemRaw[];
     constexpr int GW = Group::W;
     constexpr int GROUPS = THREADS / GW;
     int* E = reinterpret_cast<int*>(smemRaw);              // [groups][CAP]
-    int* ctl = E + GROUPS * CAP;                            // [groups][SEED_CTL]
+    int* ctl = E + GROUPS * CAP;                            // [groups][seed_ctl_words(GW)]
     const int g = threadIdx.x / GW;
-    const int slot = blockIdx.x * GROUPS + g;
-    if (slot < p.numReads) seed_plan_read<CAP, Group>(p, slot, E + g * CAP, ctl + g * SEED_CTL);
+    // every group runs, also past numReads: the warp reserves its window jobs together
+    seed_plan_read<CAP, Group>(p, blockIdx.x * GROUPS + g, E + g * CAP, ctl + g * seed_ctl_words(GW));
 }
 __global__ void win_reduce_kernel(const WinReduceParams p) {
     const int slot = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1103,19 +1123,28 @@ struct CudaBackend : Backend {
         }
         free(tileSums);
     }
-    template <int CAP, int THREADS, class Group, int GW>
+    template <int CAP, int THREADS, int GW>
     void launch_seed_plan_t(const SeedPlanParams& p) {
         constexpr int GROUPS = THREADS / GW;
-        const size_t smem = (size_t)GROUPS * ((size_t)CAP + SEED_CTL) * sizeof(int);
+        const size_t smem = (size_t)GROUPS * ((size_t)CAP + seed_ctl_words(GW)) * sizeof(int);
         if (smem > 48 * 1024)
-            EB_CUDA(cudaFuncSetAttribute(seed_plan_kernel<CAP, THREADS, Group>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        seed_plan_kernel<CAP, THREADS, Group><<<(p.numReads + GROUPS - 1) / GROUPS, THREADS, smem, stream>>>(p);
+            EB_CUDA(cudaFuncSetAttribute(seed_plan_kernel<CAP, THREADS, CoopGroup<GW>>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        seed_plan_kernel<CAP, THREADS, CoopGroup<GW>><<<(p.numReads + GROUPS - 1) / GROUPS, THREADS, smem, stream>>>(p);
     }
     void launch_seed_plan(const SeedPlanParams& p) override {
         Scope s(this, "seed_plan");
-        if (p.level <= 0) launch_seed_plan_t<SEED_CAND_0, 128, CoopGroup8, 8>(p);
-        else if (p.level == 1) launch_seed_plan_t<SEED_CAND_1, 128, CoopGroup8, 8>(p);
-        else launch_seed_plan_t<SEED_CAND_2, 64, CoopGroup32, 32>(p);  // a warp per read, two reads per CTA
+        // a read has t + 1 <= min(maxLen / Ls, seedK + 1) seeds: groups of 16 lanes look them all up in one round
+        // when that is at most 16, whole warps otherwise (or when the read lengths are not known)
+        const bool narrow = p.maxLen > 0 && p.Ls > 0 && std::min(p.maxLen / p.Ls, p.seedK + 1) <= 16;
+        if (p.level <= 0) {
+            if (narrow) launch_seed_plan_t<SEED_CAND_0, 128, 16>(p);
+            else launch_seed_plan_t<SEED_CAND_0, 128, 32>(p);
+        } else if (p.level == 1) {
+            if (narrow) launch_seed_plan_t<SEED_CAND_1, 128, 16>(p);
+            else launch_seed_plan_t<SEED_CAND_1, 128, 32>(p);
+        } else {
+            launch_seed_plan_t<SEED_CAND_2, 64, 32>(p);  // a warp per read, two reads per CTA
+        }
         check_launch("seed_plan");
     }
     void launch_fin_count(const FinParams& p) override {

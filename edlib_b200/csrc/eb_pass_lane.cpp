@@ -339,6 +339,7 @@ void Pass::seed_stage(LaneGroup& c, int level, const std::vector<int>& in, std::
         sp.readList = dList.p;
         sp.thr = dThr.p;
         sp.numReads = g;
+        sp.maxLen = 32 * nw;
         sp.winPair = wPair.p;
         sp.winK = wK.p;
         sp.winStart = wStart.p;
@@ -872,6 +873,7 @@ int Pass::dev_enqueue_slice(int t, int nw, int firstPair, const int* listHost, i
     sp.firstPair = sl.firstPair;
     sp.thr = nullptr;
     sp.numReads = count;
+    sp.maxLen = 32 * nw;
     sp.winPair = wPair.p;
     sp.winK = wK.p;
     sp.winStart = wStart.p;
