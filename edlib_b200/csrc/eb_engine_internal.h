@@ -452,6 +452,30 @@ struct TargetHandle {
     SeedIndex idx;
 };
 
+// Window jobs of the candidate filter on the device (the job arrays of K1WParams): planned by the seed planner, which
+// counts them in `count` (zeroed by the caller), or planned on the host and uploaded (count == nullptr).
+struct WinJobs {
+    DevBuf<int> pair, k, start, len, tf;  // pair, threshold + 1, first column, columns, first tracked column (relative)
+    int cap = 0;
+    int* count = nullptr;
+    void alloc(Backend* be, int n) {
+        pair.alloc(be, n);
+        k.alloc(be, n);
+        start.alloc(be, n);
+        len.alloc(be, n);
+        tf.alloc(be, n);
+        cap = n;
+    }
+};
+// What the sweeps of window jobs record: one WinRec per job, and the end columns beyond its inline ones in ovf (counted
+// in *ovfCount, zeroed by the caller; the list is complete while the count stays <= ovfCap).
+struct WinRecords {
+    WinRec* recs;
+    Ovf* ovf;
+    int* ovfCount;
+    int ovfCap;
+};
+
 // One slice of a device-driven group: reads [first, first+count) of the group's list (pair = list[first+slot], or
 // firstPair + slot when the group is a run of consecutive pairs), its region of the end-location pool and its
 // header {end locations, reads pending, pool overflow, windows}.
@@ -614,6 +638,21 @@ struct Pass {
     SeedIndex* seedIdx = nullptr;
     SeedIndex ownIdx;
     bool seed_index(int t);
+
+    // ---- seed windows of the candidate filter: planned (seed_plan), swept (k1w), reduced per read (win_reduce) ----
+    // Planner parameters of seed level `level` over target tg; the caller adds its reads (readList / firstPair, thr,
+    // numReads, maxLen) and their plans (plan).
+    SeedPlanParams seed_plan_params(const Target& tg, int level) const;
+    // Plans the windows of sp's reads into `jobs`, with room for `cap` of them (*jobs.count zero).  hostCount: returns their
+    // number, planned again with the exact room when they did not fit.  Otherwise the number stays on the device (reads
+    // whose windows do not fit are saturated) and -1 is returned.
+    int plan_windows(SeedPlanParams sp, WinJobs& jobs, int cap, bool hostCount);
+    // Sweeps the first numJobs jobs, or (numJobs < 0) as many as *jobs.count says on the device, into `out`.
+    void sweep_windows(const Target& tg, int nw, const WinJobs& jobs, int numJobs, const WinRecords& out);
+    // Reduces the window records of the planned reads into out[numReads] (positions past KPOS in extra); rp carries
+    // the fields of the device-driven mode, or none.
+    void reduce_windows(WinReduceParams rp, const SeedPlan* plan, int numReads, const WinRecords& wr, Rec* out, int* extra,
+                        int* extraCount, int extraCap);
 
     // One group of pairs that share a target and a word class (queries <= 256 rows), on its way through
     // the host-driven stages of the distance pass.  Reads are addressed by their index `s` into `list`.

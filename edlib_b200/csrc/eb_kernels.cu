@@ -24,6 +24,7 @@
 #include <vector>
 
 #include "eb_core.h"
+#include "eb_dispatch.h"
 #include "eb_engine.h"
 
 namespace eb {
@@ -815,43 +816,40 @@ struct CudaBackend : Backend {
         EB_CUDA(cudaEventCreate(&e));
         return e;
     }
-    struct Scope {
-        CudaBackend* be;
-        Timed t;
-        Scope(CudaBackend* b, const char* name) : be(b) {
-            t.name = name;
-            t.a = be->get_event();
-            t.b = be->get_event();
-            cudaEventRecord(t.a, be->stream);
-        }
-        ~Scope() {
-            cudaEventRecord(t.b, be->stream);
-            be->timed.push_back(t);
-            be->launchCount++;
-        }
-    };
     static void check_launch(const char* what) {
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) throw std::runtime_error(std::string(what) + " launch: " + cudaGetErrorString(e));
     }
+    // Dynamic shared memory beyond the default 48 KiB needs the kernel's opt-in.  The attribute is the kernel's limit, not
+    // a switch: it is only set above 48 KiB, so it never drops below what a later launch within the default needs.
+    template <class K>
+    static cudaError_t opt_in_smem(K kernel, size_t smem) {
+        return smem > 48 * 1024 ? cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) : cudaSuccess;
+    }
+    // Every kernel launch: on the compute stream, timed under `name` (kernel_ms, kernel_report).
+    template <class... KArgs, class... Args>
+    void launch(const char* name, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, const Args&... args) {
+        EB_CUDA(opt_in_smem(kernel, smem));
+        Timed t{name, get_event(), get_event()};
+        cudaEventRecord(t.a, stream);
+        kernel<<<grid, block, smem, stream>>>(args...);
+        cudaEventRecord(t.b, stream);
+        timed.push_back(t);
+        launchCount++;
+        check_launch(name);
+    }
 
     void launch_mask(const MaskParams& p) override {
-        Scope s(this, "mask");
-        mask_kernel<<<(p.numItems + p.numQueries + W_WARPS - 1) / W_WARPS, W_WARPS * 32, 0, stream>>>(p);
-        check_launch("mask");
+        launch("mask", mask_kernel, (p.numItems + p.numQueries + W_WARPS - 1) / W_WARPS, W_WARPS * 32, 0, p);
     }
     void launch_alpha_len(const uint32_t* masks, const int* qset, const int* tset, int n, int* out) override {
-        Scope s(this, "alpha");
-        alpha_len_kernel<<<(n + 255) / 256, 256, 0, stream>>>(masks, qset, tset, n, out);
-        check_launch("alpha_len");
+        launch("alpha", alpha_len_kernel, (n + 255) / 256, 256, 0, masks, qset, tset, n, out);
     }
     void launch_encode(const EncodeParams& p) override {
-        Scope s(this, "encode");
         const uint64_t nvec = p.numBytes / 16 + 1;
         int blocks = (int)std::min<uint64_t>((nvec + 255) / 256, (uint64_t)sms * 8);
         if (blocks < 1) blocks = 1;
-        encode_kernel<<<blocks, 256, 0, stream>>>(p);
-        check_launch("encode");
+        launch("encode", encode_kernel, blocks, 256, 0, p);
     }
 
     // CTA size and dynamic shared memory of a K1 launch: four CTAs of 256 threads per SM when the
@@ -866,21 +864,10 @@ struct CudaBackend : Backend {
         *block = b;
         *smem = fixed + perThread * b;
     }
-    template <int NW, int MODE>
-    void launch_k1_t(const K1Params& p) {
-        int block;
-        size_t smem;
-        k1_block(NW, p.ncodes, p.numReads, &block, &smem);
-        if (smem > (size_t)maxSmemOptin) throw std::runtime_error("K1: alphabet too large for shared memory");
-        EB_CUDA(cudaFuncSetAttribute(k1_kernel<NW, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        dim3 grid((p.numReads + block - 1) / block, p.chunks);
-        k1_kernel<NW, MODE><<<grid, block, smem, stream>>>(p);
-        check_launch("k1");
-    }
     template <int NW>
     int k1_occupancy(int block, size_t smem) {
         int perSm = 0;
-        cudaFuncSetAttribute(k1_kernel<NW, MODE_HW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        opt_in_smem(k1_kernel<NW, MODE_HW>, smem);
         if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, k1_kernel<NW, MODE_HW>, block, smem) != cudaSuccess) perSm = 1;
         return perSm < 1 ? 1 : perSm;
     }
@@ -904,167 +891,68 @@ struct CudaBackend : Backend {
             return;
         }
         int perSm = 1;
-        switch (nw) {
-            case 1: perSm = k1_occupancy<1>(block, smem); break;
-            case 2: perSm = k1_occupancy<2>(block, smem); break;
-            case 3: perSm = k1_occupancy<3>(block, smem); break;
-            case 4: perSm = k1_occupancy<4>(block, smem); break;
-            case 5: perSm = k1_occupancy<5>(block, smem); break;
-            case 6: perSm = k1_occupancy<6>(block, smem); break;
-            case 7: perSm = k1_occupancy<7>(block, smem); break;
-            default: perSm = k1_occupancy<8>(block, smem); break;
-        }
+        with_nw(nw, [&](auto w) { perSm = k1_occupancy<decltype(w)::value>(block, smem); });
         *blockThreads = block;
         *residentCtas = perSm * sms;
         if (ncodes < 1023) shapeCache[key] = block | ((perSm * sms) << 12);
     }
-    // candidate-filter sweeps: 32- or 64-row prefixes (one or two words), HW, range recording
-    template <int NW>
-    void launch_k1_range_t(const K1Params& p) {
-        int block;
-        size_t smem;
-        k1_block(NW, p.ncodes, p.numReads, &block, &smem);
-        if (smem > (size_t)maxSmemOptin) throw std::runtime_error("K1: alphabet too large for shared memory");
-        dim3 grid((p.numReads + block - 1) / block, p.chunks);
-        EB_CUDA(cudaFuncSetAttribute(k1_kernel<NW, MODE_HW, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k1_kernel<NW, MODE_HW, true><<<grid, block, smem, stream>>>(p);
-        check_launch("k1 range");
-    }
-    template <int NW>
-    void launch_k1_m(const K1Params& p) {
-        if (p.mode == MODE_HW) launch_k1_t<NW, MODE_HW>(p);
-        else if (p.mode == MODE_SHW) launch_k1_t<NW, MODE_SHW>(p);
-        else launch_k1_t<NW, MODE_NW>(p);
-    }
-    template <int NW>
-    void launch_k1t_t(const K1Params& p) {
-        const size_t smem = (size_t)p.ncodes * NW * sizeof(uint32_t);
-        if (smem > 48 * 1024) EB_CUDA(cudaFuncSetAttribute(k1t_kernel<NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k1t_kernel<NW><<<dim3((unsigned)((p.chunks + 31) / 32), (unsigned)p.numReads), 32, smem, stream>>>(p);
-        check_launch("k1t");
-    }
     void launch_k1t(const K1Params& p, int nw) override {
-        Scope s(this, "k1");
         if (p.rangeMode || p.prefixLen > 0) throw std::runtime_error("k1t: plain sweeps only");
-        switch (nw) {
-            case 1: launch_k1t_t<1>(p); break;
-            case 2: launch_k1t_t<2>(p); break;
-            case 3: launch_k1t_t<3>(p); break;
-            case 4: launch_k1t_t<4>(p); break;
-            case 5: launch_k1t_t<5>(p); break;
-            case 6: launch_k1t_t<6>(p); break;
-            case 7: launch_k1t_t<7>(p); break;
-            case 8: launch_k1t_t<8>(p); break;
-            default: throw std::runtime_error("bad K1 word class");
-        }
+        const size_t smem = (size_t)p.ncodes * nw * sizeof(uint32_t);
+        const dim3 grid((unsigned)((p.chunks + 31) / 32), (unsigned)p.numReads);
+        with_nw(nw, [&](auto w) { launch("k1", k1t_kernel<decltype(w)::value>, grid, 32, smem, p); });
     }
     void launch_k1(const K1Params& p, int nw) override {
-        Scope s(this, p.rangeMode ? "k1_prefix" : "k1");
-        if (p.rangeMode) {
-            if ((nw != 1 && nw != 2) || p.mode != MODE_HW) throw std::runtime_error("range mode needs the 1- or 2-word HW kernel");
-            if (nw == 1) launch_k1_range_t<1>(p);
-            else launch_k1_range_t<2>(p);
+        int block;
+        size_t smem;
+        k1_block(nw, p.ncodes, p.numReads, &block, &smem);
+        if (smem > (size_t)maxSmemOptin) throw std::runtime_error("K1: alphabet too large for shared memory");
+        const dim3 grid((p.numReads + block - 1) / block, p.chunks);
+        if (p.rangeMode) {  // candidate-filter sweeps: 32- or 64-row prefixes (one or two words), HW, range recording
+            const char* bad = "range mode needs the 1- or 2-word HW kernel";
+            if (p.mode != MODE_HW) throw std::runtime_error(bad);
+            with_one_of<1, 2>(nw, bad, [&](auto w) { launch("k1_prefix", k1_kernel<decltype(w)::value, MODE_HW, true>, grid, block, smem, p); });
             return;
         }
-        switch (nw) {
-            case 1: launch_k1_m<1>(p); break;
-            case 2: launch_k1_m<2>(p); break;
-            case 3: launch_k1_m<3>(p); break;
-            case 4: launch_k1_m<4>(p); break;
-            case 5: launch_k1_m<5>(p); break;
-            case 6: launch_k1_m<6>(p); break;
-            case 7: launch_k1_m<7>(p); break;
-            case 8: launch_k1_m<8>(p); break;
-            default: throw std::runtime_error("bad K1 word class");
-        }
+        with_nw(nw, [&](auto w) {
+            with_mode(p.mode, [&](auto m) { launch("k1", k1_kernel<decltype(w)::value, decltype(m)::value>, grid, block, smem, p); });
+        });
     }
-    template <int NW, int THREADS>
-    void launch_k1w_b(const K1WParams& p, size_t smem) {
-        EB_CUDA(cudaFuncSetAttribute(k1w_kernel<NW, THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k1w_kernel<NW, THREADS><<<(p.numReads + THREADS - 1) / THREADS, THREADS, smem, stream>>>(p);
-    }
-    template <int NW>
-    void launch_k1w_t(const K1WParams& p) {
+    void launch_k1w(const K1WParams& p, int nw) override {
         int block = 128;
-        const size_t perThread = (size_t)p.ncodes * 4 * (NW + 4);
+        const size_t perThread = (size_t)p.ncodes * 4 * (nw + 4);
         while (block > 32 && perThread * block > 96 * 1024) block >>= 1;
         const size_t smem = perThread * block;
         if (smem > (size_t)maxSmemOptin) throw std::runtime_error("K1W: alphabet too large for shared memory");
-        if (block == 128) launch_k1w_b<NW, 128>(p, smem);
-        else if (block == 64) launch_k1w_b<NW, 64>(p, smem);
-        else launch_k1w_b<NW, 32>(p, smem);
-        check_launch("k1w");
+        with_nw(nw, [&](auto w) {
+            with_one_of<128, 64, 32>(block, "bad K1W CTA size", [&](auto threads) {
+                constexpr int THREADS = decltype(threads)::value;
+                launch("k1w", k1w_kernel<decltype(w)::value, THREADS>, (p.numReads + THREADS - 1) / THREADS, THREADS, smem, p);
+            });
+        });
     }
-    void launch_k1w(const K1WParams& p, int nw) override {
-        Scope s(this, "k1w");
-        switch (nw) {
-            case 1: launch_k1w_t<1>(p); break;
-            case 2: launch_k1w_t<2>(p); break;
-            case 3: launch_k1w_t<3>(p); break;
-            case 4: launch_k1w_t<4>(p); break;
-            case 5: launch_k1w_t<5>(p); break;
-            case 6: launch_k1w_t<6>(p); break;
-            case 7: launch_k1w_t<7>(p); break;
-            case 8: launch_k1w_t<8>(p); break;
-            default: throw std::runtime_error("bad K1W word class");
-        }
-    }
-    template <int NW, int MODE, bool REV, bool STORE>
-    void launch_lane_c(const LParams& p) {
+    void launch_lane(const LParams& p, int nw, int mode, bool rev, bool store) override {
         int block = 128;
-        const size_t perThread = (size_t)p.ncodes * (16 + 4 * (NW > 4 ? NW - 4 : 0));
+        const size_t perThread = (size_t)p.ncodes * (16 + 4 * (nw > 4 ? nw - 4 : 0));
         while (block > 32 && perThread * block > 96 * 1024) block >>= 1;
         const size_t smem = perThread * block;
         if (smem > (size_t)maxSmemOptin) throw std::runtime_error("lane kernel: alphabet too large for shared memory");
-        EB_CUDA(cudaFuncSetAttribute(lane_kernel<NW, MODE, REV, STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        lane_kernel<NW, MODE, REV, STORE><<<(p.numJobs + block - 1) / block, block, smem, stream>>>(p);
-        check_launch("lane");
-    }
-    template <int NW>
-    void launch_lane_t(const LParams& p, int mode, bool rev, bool store) {
-        if (store) launch_lane_c<NW, MODE_NW, false, true>(p);
-        else if (rev && mode == MODE_SHW) launch_lane_c<NW, MODE_SHW, true, false>(p);
-        else if (!rev && mode == MODE_HW) launch_lane_c<NW, MODE_HW, false, false>(p);
-        else if (!rev && mode == MODE_SHW) launch_lane_c<NW, MODE_SHW, false, false>(p);
-        else if (!rev && mode == MODE_NW) launch_lane_c<NW, MODE_NW, false, false>(p);
-        else throw std::runtime_error("unsupported lane class");
-    }
-    void launch_lane(const LParams& p, int nw, int mode, bool rev, bool store) override {
-        Scope s(this, "lane");
-        switch (nw) {
-            case 1: launch_lane_t<1>(p, mode, rev, store); break;
-            case 2: launch_lane_t<2>(p, mode, rev, store); break;
-            case 3: launch_lane_t<3>(p, mode, rev, store); break;
-            case 4: launch_lane_t<4>(p, mode, rev, store); break;
-            case 5: launch_lane_t<5>(p, mode, rev, store); break;
-            case 6: launch_lane_t<6>(p, mode, rev, store); break;
-            case 7: launch_lane_t<7>(p, mode, rev, store); break;
-            case 8: launch_lane_t<8>(p, mode, rev, store); break;
-            default: throw std::runtime_error("bad lane word class");
-        }
+        with_nw(nw, [&](auto w) {
+            with_lane_class(mode, rev, store, [&](auto c) {
+                using C = decltype(c);
+                launch("lane", lane_kernel<decltype(w)::value, C::MODE, C::REV, C::STORE>, (p.numJobs + block - 1) / block, block, smem, p);
+            });
+        });
     }
     void launch_res(const ResParams& p) override {
         if (p.numItems <= 0) return;
-        Scope s(this, "res");
-        res_kernel<<<(p.numItems + 255) / 256, 256, 0, stream>>>(p);
-        check_launch("res");
+        launch("res", res_kernel, (p.numItems + 255) / 256, 256, 0, p);
     }
     void launch_peq(const PeqParams& p) override {
-        Scope s(this, "peq");
-        peq_kernel<<<(p.numJobs + W_WARPS - 1) / W_WARPS, W_WARPS * 32, 0, stream>>>(p);
-        check_launch("peq");
+        launch("peq", peq_kernel, (p.numJobs + W_WARPS - 1) / W_WARPS, W_WARPS * 32, 0, p);
     }
     void launch_w(const WParams& p, int R) override {
-        Scope s(this, "w");
-        const int blocks = (p.numJobs + W_WARPS - 1) / W_WARPS;
-        switch (R) {
-            case 1: w_kernel<1><<<blocks, W_WARPS * 32, 0, stream>>>(p); break;
-            case 2: w_kernel<2><<<blocks, W_WARPS * 32, 0, stream>>>(p); break;
-            case 4: w_kernel<4><<<blocks, W_WARPS * 32, 0, stream>>>(p); break;
-            case 8: w_kernel<8><<<blocks, W_WARPS * 32, 0, stream>>>(p); break;
-            default: throw std::runtime_error("bad W chunk size");
-        }
-        check_launch("w");
+        with_r(R, [&](auto r) { launch("w", w_kernel<decltype(r)::value>, (p.numJobs + W_WARPS - 1) / W_WARPS, W_WARPS * 32, 0, p); });
     }
     static size_t band_smem(int NB, int ncodes) { return (size_t)ncodes * (4 * NB + BAND_SLACK) * 4 * BAND_THREADS; }
     int band_max_blocks(int ncodes) override {
@@ -1072,111 +960,45 @@ struct CudaBackend : Backend {
         while (nb < 8 && band_smem(nb + 1, ncodes) <= (size_t)110 * 1024) ++nb;  // two CTAs per SM at least
         return nb;
     }
-    template <int NB>
-    void launch_band_t(const WParams& p, int ncodes) {
-        const size_t smem = band_smem(NB, ncodes);
-        EB_CUDA(cudaFuncSetAttribute(band_kernel<NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        band_kernel<NB><<<(p.numJobs + BAND_THREADS - 1) / BAND_THREADS, BAND_THREADS, smem, stream>>>(p, ncodes);
-    }
     void launch_band(const WParams& p, int NB, int ncodes) override {
-        Scope s(this, "band");
-        switch (NB) {
-            case 1: launch_band_t<1>(p, ncodes); break;
-            case 2: launch_band_t<2>(p, ncodes); break;
-            case 3: launch_band_t<3>(p, ncodes); break;
-            case 4: launch_band_t<4>(p, ncodes); break;
-            case 5: launch_band_t<5>(p, ncodes); break;
-            case 6: launch_band_t<6>(p, ncodes); break;
-            case 7: launch_band_t<7>(p, ncodes); break;
-            case 8: launch_band_t<8>(p, ncodes); break;
-            default: throw std::runtime_error("bad band window size");
-        }
-        check_launch("band");
+        with_nb(NB, [&](auto nb) {
+            launch("band", band_kernel<decltype(nb)::value>, (p.numJobs + BAND_THREADS - 1) / BAND_THREADS, BAND_THREADS, band_smem(NB, ncodes), p,
+                   ncodes);
+        });
     }
-    void launch_seed_count(const SeedIndexParams& p) override {
-        Scope s(this, "seed_count");
-        seed_count_kernel<<<(p.numPos + 255) / 256, 256, 0, stream>>>(p);
-        check_launch("seed_count");
-    }
-    void launch_seed_fill(const SeedIndexParams& p) override {
-        Scope s(this, "seed_fill");
-        seed_fill_kernel<<<(p.numPos + 255) / 256, 256, 0, stream>>>(p);
-        check_launch("seed_fill");
-    }
+    void launch_seed_count(const SeedIndexParams& p) override { launch("seed_count", seed_count_kernel, (p.numPos + 255) / 256, 256, 0, p); }
+    void launch_seed_fill(const SeedIndexParams& p) override { launch("seed_fill", seed_fill_kernel, (p.numPos + 255) / 256, 256, 0, p); }
     void launch_scan(int* data, int count) override {
         const int numTiles = (count + SCAN_TILE - 1) / SCAN_TILE;
         int* tileSums = static_cast<int*>(alloc((size_t)numTiles * sizeof(int)));
-        {
-            Scope s(this, "scan");
-            scan_tile_sums_kernel<<<numTiles, SCAN_THREADS, 0, stream>>>(data, count, tileSums);
-            check_launch("scan tile sums");
-        }
-        {
-            Scope s(this, "scan");
-            scan_top_kernel<<<1, 1024, 0, stream>>>(tileSums, numTiles, data + count);
-            check_launch("scan top");
-        }
-        {
-            Scope s(this, "scan");
-            scan_apply_kernel<<<numTiles, SCAN_THREADS, 0, stream>>>(data, count, tileSums);
-            check_launch("scan apply");
-        }
+        launch("scan", scan_tile_sums_kernel, numTiles, SCAN_THREADS, 0, data, count, tileSums);
+        launch("scan", scan_top_kernel, 1, 1024, 0, tileSums, numTiles, data + count);
+        launch("scan", scan_apply_kernel, numTiles, SCAN_THREADS, 0, data, count, tileSums);
         free(tileSums);
     }
     template <int CAP, int THREADS, int GW>
     void launch_seed_plan_t(const SeedPlanParams& p) {
         constexpr int GROUPS = THREADS / GW;
         const size_t smem = (size_t)GROUPS * ((size_t)CAP + seed_ctl_words(GW)) * sizeof(int);
-        if (smem > 48 * 1024)
-            EB_CUDA(cudaFuncSetAttribute(seed_plan_kernel<CAP, THREADS, CoopGroup<GW>>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        seed_plan_kernel<CAP, THREADS, CoopGroup<GW>><<<(p.numReads + GROUPS - 1) / GROUPS, THREADS, smem, stream>>>(p);
+        launch("seed_plan", seed_plan_kernel<CAP, THREADS, CoopGroup<GW>>, (p.numReads + GROUPS - 1) / GROUPS, THREADS, smem, p);
     }
     void launch_seed_plan(const SeedPlanParams& p) override {
-        Scope s(this, "seed_plan");
         // a read has t + 1 <= min(maxLen / Ls, seedK + 1) seeds: groups of 16 lanes look them all up in one round
         // when that is at most 16, whole warps otherwise (or when the read lengths are not known)
         const bool narrow = p.maxLen > 0 && p.Ls > 0 && std::min(p.maxLen / p.Ls, p.seedK + 1) <= 16;
-        if (p.level <= 0) {
-            if (narrow) launch_seed_plan_t<SEED_CAND_0, 128, 16>(p);
-            else launch_seed_plan_t<SEED_CAND_0, 128, 32>(p);
-        } else if (p.level == 1) {
-            if (narrow) launch_seed_plan_t<SEED_CAND_1, 128, 16>(p);
-            else launch_seed_plan_t<SEED_CAND_1, 128, 32>(p);
-        } else {
-            launch_seed_plan_t<SEED_CAND_2, 64, 32>(p);  // a warp per read, two reads per CTA
-        }
-        check_launch("seed_plan");
+        with_seed_cap(p.level, [&](auto cap) {
+            constexpr int CAP = decltype(cap)::value;
+            if constexpr (CAP == SEED_CAND_2) launch_seed_plan_t<CAP, 64, 32>(p);  // the last level: a warp per read, two reads per CTA
+            else if (narrow) launch_seed_plan_t<CAP, 128, 16>(p);
+            else launch_seed_plan_t<CAP, 128, 32>(p);
+        });
     }
-    void launch_fin_count(const FinParams& p) override {
-        Scope s(this, "fin_count");
-        fin_count_kernel<<<(p.numReads + 255) / 256, 256, 0, stream>>>(p);
-        check_launch("fin_count");
-    }
-    void launch_fin_fill(const FinParams& p) override {
-        Scope s(this, "fin_fill");
-        fin_fill_kernel<<<(p.numReads + 255) / 256, 256, 0, stream>>>(p);
-        check_launch("fin_fill");
-    }
-    void launch_qalpha(const QAlphaParams& p) override {
-        Scope s(this, "qalpha");
-        qalpha_kernel<<<(p.numQueries + 7) / 8, 256, 0, stream>>>(p);
-        check_launch("qalpha");
-    }
-    void launch_win_reduce(const WinReduceParams& p) override {
-        Scope s(this, "win_reduce");
-        win_reduce_kernel<<<(p.numReads + 127) / 128, 128, 0, stream>>>(p);
-        check_launch("win_reduce");
-    }
-    void launch_split(const SplitParams& p) override {
-        Scope s(this, "split");
-        split_kernel<<<(p.numNodes + 63) / 64, 64, 0, stream>>>(p);
-        check_launch("split");
-    }
-    void launch_traceback(const TbParams& p) override {
-        Scope s(this, "traceback");
-        traceback_kernel<<<(p.numJobs + 127) / 128, 128, 0, stream>>>(p);
-        check_launch("traceback");
-    }
+    void launch_fin_count(const FinParams& p) override { launch("fin_count", fin_count_kernel, (p.numReads + 255) / 256, 256, 0, p); }
+    void launch_fin_fill(const FinParams& p) override { launch("fin_fill", fin_fill_kernel, (p.numReads + 255) / 256, 256, 0, p); }
+    void launch_qalpha(const QAlphaParams& p) override { launch("qalpha", qalpha_kernel, (p.numQueries + 7) / 8, 256, 0, p); }
+    void launch_win_reduce(const WinReduceParams& p) override { launch("win_reduce", win_reduce_kernel, (p.numReads + 127) / 128, 128, 0, p); }
+    void launch_split(const SplitParams& p) override { launch("split", split_kernel, (p.numNodes + 63) / 64, 64, 0, p); }
+    void launch_traceback(const TbParams& p) override { launch("traceback", traceback_kernel, (p.numJobs + 127) / 128, 128, 0, p); }
     void reset_timing() override {
         for (auto& t : timed) {
             pool.push_back(t.a);

@@ -105,8 +105,9 @@ bool Pass::seed_index(int t) {
     return ok;
 }
 
-static void fill_seed_plan(SeedPlanParams& sp, const Prepared* p, const Target& tg, const SeedIndex& sx, int level,
-                           const EngineTunables& tun) {
+SeedPlanParams Pass::seed_plan_params(const Target& tg, int level) const {
+    const SeedIndex& sx = *seedIdx;
+    SeedPlanParams sp;
     memset(&sp, 0, sizeof(sp));
     sp.tcodes = p->dSeq.p + tg.off;
     sp.n = tg.len;
@@ -124,6 +125,67 @@ static void fill_seed_plan(SeedPlanParams& sp, const Prepared* p, const Target& 
     sp.maxBucket = std::min(tun.filterSeedBucket << (1 + 3 * level), 8192);  // shorter seeds: longer index ranges are normal
     sp.level = level;
     sp.spread = tun.filterSpread;
+    return sp;
+}
+
+int Pass::plan_windows(SeedPlanParams sp, WinJobs& jobs, int cap, bool hostCount) {
+    for (;;) {
+        jobs.alloc(be, cap);
+        sp.winPair = jobs.pair.p;
+        sp.winK = jobs.k.p;
+        sp.winStart = jobs.start.p;
+        sp.winLen = jobs.len.p;
+        sp.winTf = jobs.tf.p;
+        sp.winCap = cap;
+        sp.winCount = jobs.count;
+        be->launch_seed_plan(sp);
+        if (!hostCount) return -1;
+        int V = 0;
+        be->d2h(&V, jobs.count, sizeof(int));
+        stats.d2hBytes += 4;
+        if (V <= cap) return V;
+        cap = V;  // window list overflow: plan again with the exact size
+        be->zero(jobs.count, sizeof(int));
+    }
+}
+
+void Pass::sweep_windows(const Target& tg, int nw, const WinJobs& jobs, int numJobs, const WinRecords& out) {
+    K1WParams wp;
+    memset(&wp, 0, sizeof(wp));
+    wp.tcodes = p->dSeq.p + tg.off;
+    wp.qcodes = p->dSeq.p;
+    wp.qoff = p->dQoff.p;
+    wp.qlen = p->dQlen.p;
+    wp.readList = jobs.pair.p;
+    wp.kInit = jobs.k.p;
+    wp.winStart = jobs.start.p;
+    wp.winLen = jobs.len.p;
+    wp.trackFrom = jobs.tf.p;
+    wp.numReads = numJobs < 0 ? jobs.cap : numJobs;
+    wp.countPtr = numJobs < 0 ? jobs.count : nullptr;
+    wp.checkAfter = tun.windowCheckAfter;
+    wp.ncodes = p->ncodes;
+    wp.eqtab = p->hasEq ? p->dEqtab.p : nullptr;
+    wp.recs = out.recs;
+    wp.ovf = out.ovf;
+    wp.ovfCount = out.ovfCount;
+    wp.ovfCap = out.ovfCap;
+    be->launch_k1w(wp, nw);
+}
+
+void Pass::reduce_windows(WinReduceParams rp, const SeedPlan* plan, int numReads, const WinRecords& wr, Rec* out, int* extra,
+                          int* extraCount, int extraCap) {
+    rp.plan = plan;
+    rp.winRecs = wr.recs;
+    rp.numReads = numReads;
+    rp.out = out;
+    rp.extra = extra;
+    rp.extraCount = extraCount;
+    rp.extraCap = extraCap;
+    rp.ovf = wr.ovf;
+    rp.ovfCount = wr.ovfCount;
+    rp.ovfCap = wr.ovfCap;
+    be->launch_win_reduce(rp);
 }
 
 // Chunk geometry: a HW sweep may be cut into target chunks (each re-started 2*m columns
@@ -304,8 +366,7 @@ void Pass::seed_stage(LaneGroup& c, int level, const std::vector<int>& in, std::
         next = in;
         return;
     }
-    const SeedIndex& sx = *seedIdx;
-    const int L = sx.Ls[level];
+    const int L = seedIdx->Ls[level];
     // every read of `in` gets a slot; thr < 0 marks the ones this stage cannot help (the kernel skips them)
     const std::vector<int>& cand = in;
     const int g = (int)cand.size();
@@ -323,37 +384,19 @@ void Pass::seed_stage(LaneGroup& c, int level, const std::vector<int>& in, std::
     dList.upload(rl.p, g);
     dThr.upload(hThr.p, g);
     DevBuf<SeedPlan> dPlan(be, g);
-    DevBuf<int> wPair, wK, wStart, wLen, wTf;
     // room for the window jobs: sized from what the previous pass of this level needed per read
     int& perRead = eng.scratch.seedWindowsPerRead[level];
-    int cap = (int)std::min<long long>((long long)g * std::max(perRead + 2, level == 0 ? 8 : level == 1 ? 96 : level == 2 ? 400 : 1500) + 4096, 1LL << 28), V = 0;
-    for (;;) {
-        wPair.alloc(be, cap);
-        wK.alloc(be, cap);
-        wStart.alloc(be, cap);
-        wLen.alloc(be, cap);
-        wTf.alloc(be, cap);
-        be->zero(dCount.p, sizeof(int));
-        SeedPlanParams sp;
-        fill_seed_plan(sp, p, tg, sx, level, tun);
-        sp.readList = dList.p;
-        sp.thr = dThr.p;
-        sp.numReads = g;
-        sp.maxLen = 32 * nw;
-        sp.winPair = wPair.p;
-        sp.winK = wK.p;
-        sp.winStart = wStart.p;
-        sp.winLen = wLen.p;
-        sp.winTf = wTf.p;
-        sp.winCap = cap;
-        sp.winCount = dCount.p;
-        sp.plan = dPlan.p;
-        be->launch_seed_plan(sp);
-        dCount.download(&V, 1);
-        stats.d2hBytes += 4;
-        if (V <= cap) break;
-        cap = V;  // window list overflow: repeat with the exact size
-    }
+    const int cap = (int)std::min<long long>((long long)g * std::max(perRead + 2, level == 0 ? 8 : level == 1 ? 96 : level == 2 ? 400 : 1500) + 4096, 1LL << 28);
+    SeedPlanParams sp = seed_plan_params(tg, level);
+    sp.readList = dList.p;
+    sp.thr = dThr.p;
+    sp.numReads = g;
+    sp.maxLen = 32 * nw;
+    sp.plan = dPlan.p;
+    WinJobs jobs;
+    jobs.count = dCount.p;
+    be->zero(dCount.p, sizeof(int));
+    const int V = plan_windows(sp, jobs, cap, true);
     perRead = (int)(((long long)V + g - 1) / g);
     stats.filterWindows += V;
     trace.mark("filter: seeds planned");
@@ -363,28 +406,8 @@ void Pass::seed_stage(LaneGroup& c, int level, const std::vector<int>& in, std::
     DevBuf<Ovf> dOvf(be, (size_t)ovfCap);
     DevBuf<int> dOvfCount(be, 1);
     be->zero(dOvfCount.p, sizeof(int));
-    if (V > 0) {
-        K1WParams wp;
-        memset(&wp, 0, sizeof(wp));
-        wp.tcodes = p->dSeq.p + tg.off;
-        wp.qcodes = p->dSeq.p;
-        wp.qoff = p->dQoff.p;
-        wp.qlen = p->dQlen.p;
-        wp.readList = wPair.p;
-        wp.kInit = wK.p;
-        wp.winStart = wStart.p;
-        wp.winLen = wLen.p;
-        wp.trackFrom = wTf.p;
-        wp.numReads = V;
-        wp.checkAfter = tun.windowCheckAfter;
-        wp.ncodes = p->ncodes;
-        wp.eqtab = nullptr;
-        wp.recs = dWinRecs.p;
-        wp.ovf = dOvf.p;
-        wp.ovfCount = dOvfCount.p;
-        wp.ovfCap = ovfCap;
-        be->launch_k1w(wp, nw);
-    }
+    const WinRecords wr{dWinRecs.p, dOvf.p, dOvfCount.p, ovfCap};
+    if (V > 0) sweep_windows(tg, nw, jobs, V, wr);
     DevBuf<Rec> dOut(be, g);
     int extraCap = g / 4 + 16384;
     DevBuf<int> dExtra;
@@ -392,19 +415,7 @@ void Pass::seed_stage(LaneGroup& c, int level, const std::vector<int>& in, std::
     for (;;) {
         dExtra.alloc(be, (size_t)extraCap);
         be->zero(dCount.p, sizeof(int));
-        WinReduceParams rp;
-        memset(&rp, 0, sizeof(rp));
-        rp.plan = dPlan.p;
-        rp.winRecs = dWinRecs.p;
-        rp.numReads = g;
-        rp.out = dOut.p;
-        rp.extra = dExtra.p;
-        rp.extraCount = dCount.p;
-        rp.extraCap = extraCap;
-        rp.ovf = dOvf.p;
-        rp.ovfCount = dOvfCount.p;
-        rp.ovfCap = ovfCap;
-        be->launch_win_reduce(rp);
+        reduce_windows(WinReduceParams{}, dPlan.p, g, wr, dOut.p, dExtra.p, dCount.p, extraCap);
         dCount.download(&nExtra, 1);
         if (nExtra <= extraCap) break;
         extraCap = nExtra;  // the extra list ran over (repeat-rich reads): reduce again with the exact size
@@ -615,37 +626,19 @@ void Pass::prefix_stage(LaneGroup& c, int P, int K0, const std::vector<int>& in,
     }
     if (V == 0) return;
     // Whole reads over their windows, one window per thread (k1w_kernel).
-    DevBuf<int> dPair(be, V), dK(be, V), dWs(be, V), dLen(be, V), dTf(be, V);
-    dPair.upload(vPair.data(), V);
-    dK.upload(vK.data(), V);
-    dWs.upload(vWs.data(), V);
-    dLen.upload(vLen.data(), V);
-    dTf.upload(vTf.data(), V);
+    WinJobs jobs;
+    jobs.alloc(be, V);
+    jobs.pair.upload(vPair.data(), V);
+    jobs.k.upload(vK.data(), V);
+    jobs.start.upload(vWs.data(), V);
+    jobs.len.upload(vLen.data(), V);
+    jobs.tf.upload(vTf.data(), V);
     DevBuf<WinRec> dRecs(be, V);
     const int ovfCap = (int)std::min<long long>((long long)V / 8 + 65536, 1 << 24);
     DevBuf<Ovf> dOvf(be, (size_t)ovfCap);
     DevBuf<int> dOvfCount(be, 1);
     be->zero(dOvfCount.p, sizeof(int));
-    K1WParams wp;
-    memset(&wp, 0, sizeof(wp));
-    wp.tcodes = p->dSeq.p + tg.off;
-    wp.qcodes = p->dSeq.p;
-    wp.qoff = p->dQoff.p;
-    wp.qlen = p->dQlen.p;
-    wp.readList = dPair.p;
-    wp.kInit = dK.p;
-    wp.winStart = dWs.p;
-    wp.winLen = dLen.p;
-    wp.trackFrom = dTf.p;
-    wp.numReads = V;
-    wp.checkAfter = tun.windowCheckAfter;
-    wp.ncodes = p->ncodes;
-    wp.eqtab = p->hasEq ? p->dEqtab.p : nullptr;
-    wp.recs = dRecs.p;
-    wp.ovf = dOvf.p;
-    wp.ovfCount = dOvfCount.p;
-    wp.ovfCap = ovfCap;
-    be->launch_k1w(wp, nw);
+    sweep_windows(tg, nw, jobs, V, WinRecords{dRecs.p, dOvf.p, dOvfCount.p, ovfCap});
     std::vector<WinRec> rv(V);
     dRecs.download(rv.data(), V);
     int nOvf = 0;
@@ -838,7 +831,6 @@ void Pass::dev_begin(int maxSlices) {
 int Pass::dev_enqueue_slice(int t, int nw, int firstPair, const int* listHost, int first, int count) {
     const Target& tg = p->tg[t];
     if (!seed_index(t) || seedIdx->Ls[0] <= 0) throw std::runtime_error("internal: device stage without a seed index");
-    const SeedIndex& sx = *seedIdx;
     const int si = (int)slices.size();
     DevSlice sl;
     sl.t = t;
@@ -862,67 +854,29 @@ int Pass::dev_enqueue_slice(int t, int nw, int firstPair, const int* listHost, i
     const int ovfCap = cap / 8 + 65536;
     DevBuf<Ovf> dOvf(be, (size_t)ovfCap);
     DevBuf<SeedPlan> dPlan(be, count);
-    DevBuf<int> wPair(be, cap), wK(be, cap), wStart(be, cap), wLen(be, cap), wTf(be, cap);
     DevBuf<WinRec> dWinRecs(be, cap);
     DevBuf<Rec> dOut(be, count);
-    DevBuf<int> dExtra(be, extraCap), dCnt32(be, (size_t)count + 1), dCtr(be, 3);
+    DevBuf<int> dExtra(be, extraCap), dCnt32(be, (size_t)count + 1), dCtr(be, 3);  // counters: windows, extra list, overflow list
     be->zero(dCtr.p, 3 * sizeof(int));
-    SeedPlanParams sp;
-    fill_seed_plan(sp, p, tg, sx, 0, tun);
+    SeedPlanParams sp = seed_plan_params(tg, 0);
     sp.readList = dList;
     sp.firstPair = sl.firstPair;
-    sp.thr = nullptr;
     sp.numReads = count;
     sp.maxLen = 32 * nw;
-    sp.winPair = wPair.p;
-    sp.winK = wK.p;
-    sp.winStart = wStart.p;
-    sp.winLen = wLen.p;
-    sp.winTf = wTf.p;
-    sp.winCap = cap;
-    sp.winCount = dCtr.p;
     sp.plan = dPlan.p;
-    be->launch_seed_plan(sp);
-    K1WParams wp;
-    memset(&wp, 0, sizeof(wp));
-    wp.tcodes = p->dSeq.p + tg.off;
-    wp.qcodes = p->dSeq.p;
-    wp.qoff = p->dQoff.p;
-    wp.qlen = p->dQlen.p;
-    wp.readList = wPair.p;
-    wp.kInit = wK.p;
-    wp.winStart = wStart.p;
-    wp.winLen = wLen.p;
-    wp.trackFrom = wTf.p;
-    wp.numReads = cap;
-    wp.countPtr = dCtr.p;
-    wp.checkAfter = tun.windowCheckAfter;
-    wp.ncodes = p->ncodes;
-    wp.eqtab = nullptr;
-    wp.recs = dWinRecs.p;
-    wp.ovf = dOvf.p;
-    wp.ovfCount = dCtr.p + 2;
-    wp.ovfCap = ovfCap;
-    be->launch_k1w(wp, nw);
-    WinReduceParams rp;
-    memset(&rp, 0, sizeof(rp));
-    rp.plan = dPlan.p;
-    rp.winRecs = dWinRecs.p;
-    rp.numReads = count;
-    rp.out = dOut.p;
-    rp.extra = dExtra.p;
-    rp.extraCount = dCtr.p + 1;
-    rp.extraCap = extraCap;
-    rp.ovf = dOvf.p;
-    rp.ovfCount = dCtr.p + 2;
-    rp.ovfCap = ovfCap;
+    WinJobs jobs;
+    jobs.count = dCtr.p;
+    plan_windows(sp, jobs, cap, false);
+    const WinRecords wr{dWinRecs.p, dOvf.p, dCtr.p + 2, ovfCap};
+    sweep_windows(tg, nw, jobs, -1, wr);
+    WinReduceParams rp{};
     rp.leftover = dLeft.p;
     rp.leftoverCount = dLeftCount.p;
     rp.readList = dList;
     rp.firstPair = sl.firstPair;
     rp.qlen = p->dQlen.p;
     rp.kBound = k;
-    be->launch_win_reduce(rp);
+    reduce_windows(rp, dPlan.p, count, wr, dOut.p, dExtra.p, dCtr.p + 1, extraCap);
     FinParams fp;
     memset(&fp, 0, sizeof(fp));
     fp.recs = dOut.p;

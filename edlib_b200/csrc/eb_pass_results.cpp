@@ -45,8 +45,7 @@ void Pass::long_hw_distance(const std::vector<int>& pairs) {
             rest.swap(cur);
         }
         for (int thrCap = 64; !cur.empty(); thrCap *= 2) {
-            const SeedIndex& sx = *seedIdx;
-            const int L = sx.Ls[0];
+            const int L = seedIdx->Ls[0];
             std::vector<int> in, rl, thr, top;
             for (int s : cur) {
                 const int m = p->qlen[list[s]];
@@ -68,59 +67,28 @@ void Pass::long_hw_distance(const std::vector<int>& pairs) {
             dList.upload(rl.data(), g);
             dThr.upload(thr.data(), g);
             DevBuf<SeedPlan> dPlan(be, g);
-            DevBuf<int> wPair, wK, wStart, wLen, wTf;
-            int cap = g * 64 + 1024, V = 0;
-            for (;;) {
-                wPair.alloc(be, cap);
-                wK.alloc(be, cap);
-                wStart.alloc(be, cap);
-                wLen.alloc(be, cap);
-                wTf.alloc(be, cap);
-                be->zero(dCount.p, sizeof(int));
-                SeedPlanParams sp;
-                memset(&sp, 0, sizeof(sp));
-                sp.tcodes = p->dSeq.p + tg.off;
-                sp.n = n;
-                sp.qcodes = p->dSeq.p;
-                sp.qoff = p->dQoff.p;
-                sp.qlen = p->dQlen.p;
-                sp.readList = dList.p;
-                sp.thr = dThr.p;
-                sp.kBound = k;
-                sp.seedK = tun.longSeedMaxK;
-                sp.numReads = g;
-                sp.Ls = L;
-                sp.Lidx = sx.Lidx;
-                sp.sigma = sx.sigma;
-                sp.numKeys = sx.numKeys;
-                sp.bucketStart = sx.bucketStart.p;
-                sp.positions = sx.positions.p;
-                sp.maxBucket = tun.filterSeedBucket * 8;
-                sp.level = SEED_LEVELS - 1;  // the largest candidate capacity
-                sp.spread = tun.filterSpread;
-                sp.winPair = wPair.p;
-                sp.winK = wK.p;
-                sp.winStart = wStart.p;
-                sp.winLen = wLen.p;
-                sp.winTf = wTf.p;
-                sp.winCap = cap;
-                sp.winCount = dCount.p;
-                sp.plan = dPlan.p;
-                be->launch_seed_plan(sp);
-                dCount.download(&V, 1);
-                if (V <= cap) break;
-                cap = V;
-            }
+            SeedPlanParams sp = seed_plan_params(tg, 0);
+            sp.readList = dList.p;
+            sp.thr = dThr.p;
+            sp.seedK = tun.longSeedMaxK;
+            sp.numReads = g;
+            sp.maxBucket = tun.filterSeedBucket * 8;
+            sp.level = SEED_LEVELS - 1;  // the largest candidate capacity
+            sp.plan = dPlan.p;
+            WinJobs jobs;
+            jobs.count = dCount.p;
+            be->zero(dCount.p, sizeof(int));
+            const int V = plan_windows(sp, jobs, g * 64 + 1024, true);
             std::vector<SeedPlan> plan(g);
             dPlan.download(plan.data(), g);
             std::vector<int> hStart(V), hLen(V), hTf(V);
             if (V) {
-                wStart.download(hStart.data(), V);
-                wLen.download(hLen.data(), V);
-                wTf.download(hTf.data(), V);
+                jobs.start.download(hStart.data(), V);
+                jobs.len.download(hLen.data(), V);
+                jobs.tf.download(hTf.data(), V);
             }
             stats.filterWindows += V;
-            stats.d2hBytes += 4 + 16LL * g + 12LL * V;
+            stats.d2hBytes += 16LL * g + 12LL * V;
             std::vector<WTask> tasks;
             std::vector<int> taskFirst(g + 1, 0);
             for (int i = 0; i < g; ++i) {

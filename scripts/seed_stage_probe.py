@@ -8,7 +8,7 @@
              `seed_plan` under that name (the other reads then take the plain sweep, so that run's step time means
              nothing): the difference is what the later levels cost.
   --cpu      a numpy pass over the same reads and genome that counts, for the level-0 seeds of every read (the engine's
-             rules: eb_pass_lane.cpp build_seed_index / fill_seed_plan, eb_core.h seed_plan_read), how often each path
+             rules: eb_pass_lane.cpp build_seed_index / Pass::seed_plan_params, eb_core.h seed_plan_read), how often each path
              of the planning kernel runs: index range sizes, long ranges (> 4 entries, walked by the whole group),
              candidates per read, reads over 32 candidates (the bitonic sort) and saturated reads.  Needs no GPU.
 """
@@ -96,7 +96,7 @@ def cpu_run():
         code[ch] = i
     g = code[target]
     sigma = 4
-    # the engine's level-0 geometry for this target (build_seed_index / fill_seed_plan / seed_threshold, defaults)
+    # the engine's level-0 geometry for this target (build_seed_index / Pass::seed_plan_params / seed_threshold, defaults)
     L0, v = 4, float(sigma) ** 4
     while v < 4.0 * n and L0 < 32:
         v *= sigma

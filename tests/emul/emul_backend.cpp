@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "eb_core.h"
+#include "eb_dispatch.h"
 #include "eb_engine.h"
 #include "host_warp.h"
 
@@ -85,18 +86,11 @@ void emul_k1w(const K1WParams& p) {
     for (int slot = 0; slot < numJobs; ++slot) k1w_thread<NW>(p, slot, acc);
 }
 
-template <int NW>
-void emul_lane(const LParams& p, int mode, bool rev, bool store) {
+template <int NW, int MODE, bool REV, bool STORE>
+void emul_lane(const LParams& p) {
     HostPeqAcc<NW> acc;
     acc.w.assign((size_t)p.ncodes * NW, 0);
-    for (int j = 0; j < p.numJobs; ++j) {
-        if (store) lane_job<NW, MODE_NW, false, true>(p, j, acc);
-        else if (rev && mode == MODE_SHW) lane_job<NW, MODE_SHW, true, false>(p, j, acc);
-        else if (!rev && mode == MODE_HW) lane_job<NW, MODE_HW, false, false>(p, j, acc);
-        else if (!rev && mode == MODE_SHW) lane_job<NW, MODE_SHW, false, false>(p, j, acc);
-        else if (!rev && mode == MODE_NW) lane_job<NW, MODE_NW, false, false>(p, j, acc);
-        else throw std::runtime_error("unsupported lane class");
-    }
+    for (int j = 0; j < p.numJobs; ++j) lane_job<NW, MODE, REV, STORE>(p, j, acc);
 }
 
 // Window of the profile of one emulated band thread: plain array [code][slot].
@@ -179,11 +173,9 @@ struct EmulBackend : Backend {
         ++launchesCount;
         std::vector<int> E(SEED_CAND_2);
         int ctl[SEED_CTL];
-        for (int i = p.numReads - 1; i >= 0; --i) {
-            if (p.level <= 0) seed_plan_read<SEED_CAND_0, CoopSerial>(p, i, E.data(), ctl);
-            else if (p.level == 1) seed_plan_read<SEED_CAND_1, CoopSerial>(p, i, E.data(), ctl);
-            else seed_plan_read<SEED_CAND_2, CoopSerial>(p, i, E.data(), ctl);
-        }
+        with_seed_cap(p.level, [&](auto cap) {
+            for (int i = p.numReads - 1; i >= 0; --i) seed_plan_read<decltype(cap)::value, CoopSerial>(p, i, E.data(), ctl);
+        });
     }
     void launch_fin_count(const FinParams& p) override {
         ++launchesCount;
@@ -209,59 +201,24 @@ struct EmulBackend : Backend {
     }
     void launch_k1t(const K1Params& p, int nw) override {
         ++launchesCount;
-        switch (nw) {
-            case 1: emul_k1t<1>(p); break;
-            case 2: emul_k1t<2>(p); break;
-            case 3: emul_k1t<3>(p); break;
-            case 4: emul_k1t<4>(p); break;
-            case 5: emul_k1t<5>(p); break;
-            case 6: emul_k1t<6>(p); break;
-            case 7: emul_k1t<7>(p); break;
-            case 8: emul_k1t<8>(p); break;
-            default: throw std::runtime_error("bad K1 word class");
-        }
+        with_nw(nw, [&](auto w) { emul_k1t<decltype(w)::value>(p); });
     }
     void launch_k1(const K1Params& p, int nw) override {
         ++launchesCount;
-        switch (nw) {
-            case 1: emul_k1<1>(p); break;
-            case 2: emul_k1<2>(p); break;
-            case 3: emul_k1<3>(p); break;
-            case 4: emul_k1<4>(p); break;
-            case 5: emul_k1<5>(p); break;
-            case 6: emul_k1<6>(p); break;
-            case 7: emul_k1<7>(p); break;
-            case 8: emul_k1<8>(p); break;
-            default: throw std::runtime_error("bad K1 word class");
-        }
+        with_nw(nw, [&](auto w) { emul_k1<decltype(w)::value>(p); });
     }
     void launch_k1w(const K1WParams& p, int nw) override {
         ++launchesCount;
-        switch (nw) {
-            case 1: emul_k1w<1>(p); break;
-            case 2: emul_k1w<2>(p); break;
-            case 3: emul_k1w<3>(p); break;
-            case 4: emul_k1w<4>(p); break;
-            case 5: emul_k1w<5>(p); break;
-            case 6: emul_k1w<6>(p); break;
-            case 7: emul_k1w<7>(p); break;
-            case 8: emul_k1w<8>(p); break;
-            default: throw std::runtime_error("bad K1W word class");
-        }
+        with_nw(nw, [&](auto w) { emul_k1w<decltype(w)::value>(p); });
     }
     void launch_lane(const LParams& p, int nw, int mode, bool rev, bool store) override {
         ++launchesCount;
-        switch (nw) {
-            case 1: emul_lane<1>(p, mode, rev, store); break;
-            case 2: emul_lane<2>(p, mode, rev, store); break;
-            case 3: emul_lane<3>(p, mode, rev, store); break;
-            case 4: emul_lane<4>(p, mode, rev, store); break;
-            case 5: emul_lane<5>(p, mode, rev, store); break;
-            case 6: emul_lane<6>(p, mode, rev, store); break;
-            case 7: emul_lane<7>(p, mode, rev, store); break;
-            case 8: emul_lane<8>(p, mode, rev, store); break;
-            default: throw std::runtime_error("bad lane word class");
-        }
+        with_nw(nw, [&](auto w) {
+            with_lane_class(mode, rev, store, [&](auto c) {
+                using C = decltype(c);
+                emul_lane<decltype(w)::value, C::MODE, C::REV, C::STORE>(p);
+            });
+        });
     }
     void launch_peq(const PeqParams& p) override {
         ++launchesCount;
@@ -270,15 +227,9 @@ struct EmulBackend : Backend {
     }
     void launch_w(const WParams& p, int R) override {
         ++launchesCount;
-        for (int j = 0; j < p.numJobs; ++j) {
-            switch (R) {
-                case 1: w_dispatch<ebhost::HostWarp, 1>(p, j); break;
-                case 2: w_dispatch<ebhost::HostWarp, 2>(p, j); break;
-                case 4: w_dispatch<ebhost::HostWarp, 4>(p, j); break;
-                case 8: w_dispatch<ebhost::HostWarp, 8>(p, j); break;
-                default: throw std::runtime_error("bad W chunk size");
-            }
-        }
+        with_r(R, [&](auto r) {
+            for (int j = 0; j < p.numJobs; ++j) w_dispatch<ebhost::HostWarp, decltype(r)::value>(p, j);
+        });
     }
     void launch_res(const ResParams& p) override {
         ++launchesCount;
@@ -287,17 +238,7 @@ struct EmulBackend : Backend {
     int band_max_blocks(int ncodes) override { return ncodes <= 64 ? 8 : 0; }
     void launch_band(const WParams& p, int NB, int ncodes) override {
         ++launchesCount;
-        switch (NB) {
-            case 1: emul_band<1>(p, ncodes); break;
-            case 2: emul_band<2>(p, ncodes); break;
-            case 3: emul_band<3>(p, ncodes); break;
-            case 4: emul_band<4>(p, ncodes); break;
-            case 5: emul_band<5>(p, ncodes); break;
-            case 6: emul_band<6>(p, ncodes); break;
-            case 7: emul_band<7>(p, ncodes); break;
-            case 8: emul_band<8>(p, ncodes); break;
-            default: throw std::runtime_error("bad band window size");
-        }
+        with_nb(NB, [&](auto nb) { emul_band<decltype(nb)::value>(p, ncodes); });
     }
     void launch_split(const SplitParams& p) override {
         ++launchesCount;
