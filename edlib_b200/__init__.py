@@ -74,9 +74,15 @@ def align(query, target, mode="NW", task="distance", k=-1, additionalEqualities=
     return _result(d, True)
 
 
-def align_batch(queries, targets, mode="NW", task="distance", k=-1, additionalEqualities=None):
+def align_batch(queries, targets, mode="NW", task="distance", k=-1, additionalEqualities=None, strands="forward"):
     """Batched `align`: `targets` is one sequence shared by all queries, or one per query (repeat the
-    same object to share its upload).  Returns one dict per query."""
+    same object to share its upload).  Returns one dict per query.
+
+    strands="both": every query is aligned as given and as its reverse complement (DNA reads from either strand,
+    IUPAC codes complemented, case kept); each dict is the better strand's result (ties: the forward one) and gains
+    "strand": "+" or "-".  Sequences must then be bytes or ASCII str: recoding them would destroy the complement."""
+    if strands not in ("forward", "both"):
+        raise ValueError("strands must be 'forward' or 'both'")
     queries = list(queries)
     shared = isinstance(targets, (bytes, bytearray, str))
     tlist = [targets] if shared else list(targets)
@@ -85,13 +91,23 @@ def align_batch(queries, targets, mode="NW", task="distance", k=-1, additionalEq
         if id(t) not in index:
             index[id(t)] = len(distinct)
             distinct.append(t)
+    if strands == "both" and not all(_is_plain(s) for s in queries + distinct):
+        raise ValueError("strands='both' needs bytes or ASCII str sequences")
     mapped, eqs = _map_to_bytes(queries + distinct, additionalEqualities)
     qs, ts = mapped[:len(queries)], mapped[len(queries):]
     per_query = [ts[0]] * len(qs) if shared else [ts[index[id(t)]] for t in tlist]
-    st, res = library().align_batch(qs, per_query, -1 if k is None else k, MODES.get(mode, 0), TASKS.get(task, 0), eqs)
+    args = (qs, per_query, -1 if k is None else k, MODES.get(mode, 0), TASKS.get(task, 0), eqs)
+    if strands == "both":
+        st, res, chosen = library().align_batch_strands(*args)
+    else:
+        (st, res), chosen = library().align_batch(*args), None
     if st != EDLIB_STATUS_OK:
         raise Exception("There was an error. (" + library().lib.edlibB200LastError().decode() + ")")
-    return [_result(d, True) for d in res]
+    out = [_result(d, True) for d in res]
+    if chosen is not None:
+        for r, s in zip(out, chosen):
+            r["strand"] = "-" if s else "+"
+    return out
 
 
 align_many = align_batch  # the name SURVEY.md 8f proposes for the batched binding entry

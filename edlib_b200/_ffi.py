@@ -122,6 +122,22 @@ class EdlibLib:
         """queries/targets: lists of bytes (targets may repeat the SAME bytes object to share it).
         Returns (status, [dict])."""
         assert self._batch is not None
+        return self._run_batch(self._batch, queries, targets, k, mode, task, equalities)
+
+    def align_batch_strands(self, queries, targets, k=-1, mode=EDLIB_MODE_NW, task=EDLIB_TASK_DISTANCE,
+                            equalities=None):
+        """edlibB200AlignBatchStrands: each query and its reverse complement, the better strand reported.
+        Returns (status, [dict], [strand]) with strand 0 (forward) or 1 (reverse complement)."""
+        assert self._batch is not None
+        fn = self.lib.edlibB200AlignBatchStrands
+        fn.restype = C.c_int
+        fn.argtypes = [C.POINTER(C.c_char_p), C.POINTER(C.c_int), C.POINTER(C.c_char_p), C.POINTER(C.c_int),
+                       C.c_int, AlignConfig, C.POINTER(AlignResult), C.POINTER(C.c_ubyte)]
+        strands = (C.c_ubyte * max(len(queries), 1))()
+        st, out = self._run_batch(lambda *a: fn(*a, strands), queries, targets, k, mode, task, equalities)
+        return st, out, [strands[i] for i in range(len(queries))]
+
+    def _run_batch(self, call, queries, targets, k, mode, task, equalities):
         n = len(queries)
         cfg, keep = make_config(k, mode, task, equalities)
         qptr = (C.c_char_p * n)(*queries)
@@ -138,7 +154,7 @@ class EdlibLib:
         tptr = (C.c_char_p * n)(*tptr_vals)
         tlen = (C.c_int * n)(*tlen_vals)
         res = (AlignResult * n)()
-        st = self._batch(qptr, qlen, tptr, tlen, n, cfg, res)
+        st = call(qptr, qlen, tptr, tlen, n, cfg, res)
         out = []
         for i in range(n):
             out.append(result_to_dict(res[i]))

@@ -137,17 +137,16 @@ EDLIB_API void edlibFreeAlignResult(EdlibAlignResult result) {
     free(result.alignment);
 }
 
-EDLIB_API int edlibAlignBatch(const char* const* queries, const int* queryLengths,
-                              const char* const* targets, const int* targetLengths,
-                              int numPairs, const EdlibAlignConfig config, EdlibAlignResult* results) {
-    if (numPairs < 0 || (numPairs > 0 && (!queries || !queryLengths || !targets || !targetLengths || !results)))
-        return EDLIB_STATUS_ERROR;
-    if (numPairs == 0) return EDLIB_STATUS_OK;
+// edlibAlignBatch and edlibB200AlignBatchStrands (strands != nullptr)
+static int align_batch_entry(const char* const* queries, const int* queryLengths, const char* const* targets,
+                             const int* targetLengths, int numPairs, const EdlibAlignConfig& config, EdlibAlignResult* results,
+                             unsigned char* strands) {
     eb::BatchInput in{queries, queryLengths, targets, targetLengths, numPairs, config};
+    in.strands = strands != nullptr;
     if (numPairs <= kSmallBatch) {
         if (SideEngine* s = side_engine_acquire()) {
             t_lastEngine = s->eng;
-            const int rc = s->eng->align_batch(in, results);
+            const int rc = s->eng->align_batch(in, results, strands);
             if (rc != EDLIB_STATUS_OK) t_lastError = s->eng->lastError;  // (copied while the engine is still ours)
             s->mu.unlock();
             return rc;
@@ -160,9 +159,28 @@ EDLIB_API int edlibAlignBatch(const char* const* queries, const int* queryLength
         return EDLIB_STATUS_ERROR;
     }
     t_lastEngine = e;
-    const int rc = e->align_batch(in, results);
+    const int rc = e->align_batch(in, results, strands);
     if (rc != EDLIB_STATUS_OK) t_lastError = e->lastError;
     return rc;
+}
+
+EDLIB_API int edlibAlignBatch(const char* const* queries, const int* queryLengths,
+                              const char* const* targets, const int* targetLengths,
+                              int numPairs, const EdlibAlignConfig config, EdlibAlignResult* results) {
+    if (numPairs < 0 || (numPairs > 0 && (!queries || !queryLengths || !targets || !targetLengths || !results)))
+        return EDLIB_STATUS_ERROR;
+    if (numPairs == 0) return EDLIB_STATUS_OK;
+    return align_batch_entry(queries, queryLengths, targets, targetLengths, numPairs, config, results, nullptr);
+}
+
+EDLIB_API int edlibB200AlignBatchStrands(const char* const* queries, const int* queryLengths,
+                                         const char* const* targets, const int* targetLengths, int numPairs,
+                                         const EdlibAlignConfig config, EdlibAlignResult* results, unsigned char* strands) {
+    if (numPairs < 0 || (numPairs > 0 && (!queries || !queryLengths || !targets || !targetLengths || !results || !strands)))
+        return EDLIB_STATUS_ERROR;
+    if (numPairs == 0) return EDLIB_STATUS_OK;
+    if (numPairs > 0x3fffffff) return EDLIB_STATUS_ERROR;  // both strands of every read are pairs of one batch
+    return align_batch_entry(queries, queryLengths, targets, targetLengths, numPairs, config, results, strands);
 }
 
 // ref edlib.cpp:146-301
@@ -311,20 +329,46 @@ EDLIB_API int edlibB200Available(void) {
     return engine_locked() ? 1 : 0;
 }
 
-EDLIB_API EdlibB200Batch* edlibB200BatchPrepare(const char* const* queries, const int* queryLengths,
-                                                const char* const* targets, const int* targetLengths,
-                                                int numPairs, const EdlibAlignConfig config) {
+static EdlibB200Batch* batch_prepare_entry(const char* const* queries, const int* queryLengths, const char* const* targets,
+                                           const int* targetLengths, int numPairs, const EdlibAlignConfig& config, bool strands) {
     std::lock_guard<std::mutex> lock(g_mu);
     eb::Engine* e = engine_locked();
-    if (!e || numPairs <= 0) return NULL;
+    if (!e || numPairs <= 0 || (strands && numPairs > 0x3fffffff)) return NULL;
     t_lastEngine = e;
     try {
         eb::BatchInput in{queries, queryLengths, targets, targetLengths, numPairs, config};
+        in.strands = strands;
         return reinterpret_cast<EdlibB200Batch*>(e->prepare(in));
     } catch (const std::exception& ex) {
         e->lastError = ex.what();
         return NULL;
     }
+}
+
+EDLIB_API EdlibB200Batch* edlibB200BatchPrepare(const char* const* queries, const int* queryLengths,
+                                                const char* const* targets, const int* targetLengths,
+                                                int numPairs, const EdlibAlignConfig config) {
+    return batch_prepare_entry(queries, queryLengths, targets, targetLengths, numPairs, config, false);
+}
+
+EDLIB_API EdlibB200Batch* edlibB200BatchPrepareStrands(const char* const* queries, const int* queryLengths,
+                                                       const char* const* targets, const int* targetLengths,
+                                                       int numPairs, const EdlibAlignConfig config) {
+    return batch_prepare_entry(queries, queryLengths, targets, targetLengths, numPairs, config, true);
+}
+
+EDLIB_API int edlibB200BatchStrands(EdlibB200Batch* batch, unsigned char* strands) {
+    std::lock_guard<std::mutex> lock(g_mu);
+    eb::Engine* e = engine_locked();
+    if (!e || !batch || !strands) return EDLIB_STATUS_ERROR;
+    t_lastEngine = e;
+    try {
+        e->strands_of(reinterpret_cast<eb::Prepared*>(batch), strands);
+    } catch (const std::exception& ex) {
+        e->lastError = ex.what();
+        return EDLIB_STATUS_ERROR;
+    }
+    return EDLIB_STATUS_OK;
 }
 
 EDLIB_API int edlibB200BatchCompute(EdlibB200Batch* batch, EdlibB200Stats* statsOut) {

@@ -270,6 +270,22 @@ EB_HD int seed_threshold(int m, int kBound, int Ls, int seedK, int excl) {
     if (t > bound) t = bound;
     return (m >= 2 * Ls && t > excl) ? t : -1;
 }
+// Cross-strand rule of one read of a strand batch (DESIGN.md section 3).  Per strand s (0: forward, 1: reverse
+// complement): done[s] -- its outcome is final, d[s] then being its distance or 0x7fffffff (none within its bound); or
+// pending, with no distance <= excl[s] (-1: nothing known) and bound[s] the largest distance that still counts.  Ties
+// go to the forward strand, so the reverse strand only counts below d[0] and the forward strand up to d[1].  Tightens
+// the bound of a pending strand and returns the strand that has lost (its outcome becomes "no alignment"), or -1.
+EB_HD int strand_rule(const bool (&done)[2], const int (&d)[2], const int (&excl)[2], int (&bound)[2]) {
+    if (done[0] && !done[1] && d[0] != 0x7fffffff) {
+        if (d[0] - 1 < bound[1]) bound[1] = d[0] - 1;
+        if (excl[1] >= bound[1]) return 1;
+    }
+    if (done[1] && !done[0] && d[1] != 0x7fffffff) {
+        if (d[1] < bound[0]) bound[0] = d[1];
+        if (excl[0] >= bound[0]) return 0;
+    }
+    return -1;
+}
 // Per read: t+1 disjoint seeds are looked up; every exact occurrence yields the expected end column
 // of the alignment it belongs to; neighbouring ones share a window (eb_core.h: seed_plan_read).
 struct SeedPlanParams {
@@ -305,6 +321,7 @@ struct SeedPlanParams {
 struct Leftover {
     int pair;
     int excl;                // no distance <= excl exists (-1: nothing known); -2: long end-location list (plain sweep)
+    int bound;               // largest distance that still counts (strand batches: capped by the other strand's distance)
 };
 enum RecState : int { REC_DONE = 100, REC_PENDING = 101 };
 // Per read: minimum over its windows -> out[slot].
@@ -312,7 +329,8 @@ enum RecState : int { REC_DONE = 100, REC_PENDING = 101 };
 //   SEED_NONE: no distance <= t exists); the host works out what happens to the read.
 //   device-driven first level (leftover != nullptr): rsv = REC_DONE (best/cnt/pos final; best = 0x7fffffff with
 //   cnt = 0 when no alignment within the caller's bound exists) or REC_PENDING, in which case the read is
-//   appended to the leftover list for the host-driven stages.
+//   appended to the leftover list for the host-driven stages.  With `strands` set nothing is appended: a pending
+//   read keeps its excl (Leftover::excl) in out.last, and fin_count_item applies the cross-strand rule.
 struct WinReduceParams {
     const SeedPlan* plan;
     const WinRec* winRecs;
@@ -332,6 +350,7 @@ struct WinReduceParams {
     int firstPair;
     const int* qlen;
     int kBound;
+    int strands;
 };
 // Device-side assembly of editDistance / endLocations of a slice of reads decided on the device (the -1 rule of
 // ref cpp:670, 681-693 included): fin_count_item -> exclusive scan of cnt32 -> fin_fill_item.
@@ -352,6 +371,11 @@ struct FinParams {
     int poolCap;
     int* header;             // [4]: total end locations, reads pending, pool overflow flag, windows planned
     const int* winCount;     // copied into header[3]
+    // strand batches: slots 2j / 2j+1 are the two strands of a read; the cross-strand rule (strand_rule) settles the
+    // loser as "no alignment", and the strands still pending are appended to the leftover list with their bounds
+    int strands;
+    Leftover* leftover;
+    int* leftoverCount;
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -422,6 +446,11 @@ struct MaskParams {
     int numQueries;
     uint32_t* masks;         // [numSets][8] 256-bit presence sets, zeroed by the host
     int unionSet;            // set that additionally receives every byte seen (or -1)
+    // strand batches (rc != nullptr): the reads are pairs 2i, implicit item q is pair 2q; every byte at offset o < rcBytes
+    // (the read block) is also written complemented to rc[rcBytes - 1 - o] (the reverse complement of the block, read
+    // i + 1 of it being pair 2i+1), and the presence set of those bytes goes to the set after the item's own
+    uint8_t* rc;
+    uint64_t rcBytes;
 };
 struct EncodeParams {
     uint8_t* data;           // encoded in place (any alignment)

@@ -1077,13 +1077,62 @@ EB_HD void win_reduce_read(const WinReduceParams& p, int slot) {
             excl = out.rsv == SEED_LONG_LIST ? -2 : (out.rsv == SEED_NONE ? pl.thr : -1);
             out.rsv = REC_PENDING;
         }
-        if (excl != -3) {
+        if (excl != -3 && p.strands) {
+            out.last = excl;  // fin_count_item applies the cross-strand rule and appends what goes on
+        } else if (excl != -3) {
             const int at = atomic_add_int(p.leftoverCount, 1);
             p.leftover[at].pair = pair;
             p.leftover[at].excl = excl;
+            p.leftover[at].bound = bound;
         }
     }
     p.out[slot] = out;
+}
+
+// Strand batches, device-driven first level: the cross-strand rule (eb_common.h: strand_rule) on the two records of the
+// read that holds `slot` (slots 2j and 2j+1 of a slice are its forward and reverse strand; win_reduce recorded a pending
+// strand's excl in its record's `last`).  Both calls of a read see the same two records and reach the same decision;
+// each acts on its own slot.  Returns whether the slot's strand has lost; `bound` receives its bound if it goes on.
+EB_HD bool strand_lost(const FinParams& p, int slot, int& bound) {
+    const int first = slot & ~1;
+    bool done[2];
+    int d[2], excl[2], bd[2];
+    for (int s = 0; s < 2; ++s) {
+        const Rec& r = p.recs[first + s];
+        const int pair = p.readList ? p.readList[first + s] : p.firstPair + first + s;
+        const int m = p.qlen[pair];
+        bd[s] = (p.kBound < 0 || p.kBound > m) ? m : p.kBound;
+        done[s] = r.rsv != REC_PENDING;
+        d[s] = done[s] ? r.best : 0x7fffffff;
+        excl[s] = done[s] ? -1 : (r.last < -1 ? -1 : r.last);  // (-2: long end-location list, nothing known)
+    }
+    int loser = strand_rule(done, d, excl, bd);
+    if (done[0] && done[1] && d[1] != 0x7fffffff) loser = d[1] < d[0] ? 0 : 1;  // both final: keep the winner's ends only
+    bound = bd[slot & 1];
+    return loser == (slot & 1);
+}
+
+// Complement of one byte of a read (a fixed involution): A<->T, C<->G and the IUPAC codes R<->Y, K<->M, B<->V, D<->H, in
+// upper and lower case; every other byte (N, S, W, non-letters) is its own complement.
+EB_HD uint8_t complement_byte(uint8_t b) {
+    const uint8_t c = b | 0x20;  // lower case of a letter; b | 0x20 == c only for b == c and b == c - 0x20
+    uint8_t o;
+    switch (c) {
+        case 'a': o = 't'; break;
+        case 't': o = 'a'; break;
+        case 'c': o = 'g'; break;
+        case 'g': o = 'c'; break;
+        case 'r': o = 'y'; break;
+        case 'y': o = 'r'; break;
+        case 'k': o = 'm'; break;
+        case 'm': o = 'k'; break;
+        case 'b': o = 'v'; break;
+        case 'v': o = 'b'; break;
+        case 'd': o = 'h'; break;
+        case 'h': o = 'd'; break;
+        default: return b;
+    }
+    return (uint8_t)(o ^ (c ^ b));  // the case of b
 }
 
 // Number of end locations a finished sweep outcome yields (the -1 rule of ref cpp:670, 681-693: the padded
@@ -1098,9 +1147,22 @@ EB_HD int hw_accepted_count(int best, int cnt, int m, int kBound, bool* minusOne
     return cnt + (*minusOne ? 1 : 0);
 }
 EB_HD void fin_count_item(const FinParams& p, int slot) {
-    const Rec r = p.recs[slot];
+    Rec r = p.recs[slot];
     const int pair = p.readList ? p.readList[slot] : p.firstPair + slot;
     int count = 0, ed = -1;
+    if (p.strands) {
+        int bound;
+        if (strand_lost(p, slot, bound)) {  // no alignment (fin_fill copies nothing of it)
+            r.best = 0x7fffffff;
+            r.cnt = 0;
+            r.rsv = REC_DONE;
+        } else if (r.rsv == REC_PENDING) {
+            const int at = atomic_add_int(p.leftoverCount, 1);
+            p.leftover[at].pair = pair;
+            p.leftover[at].excl = r.last;
+            p.leftover[at].bound = bound;
+        }
+    }
     if (r.rsv == REC_PENDING) {
         ed = -2;
         atomic_add_int(p.header + 1, 1);
@@ -1850,22 +1912,31 @@ EB_HD void split_node(const SplitParams& p, int nodeIdx) {
     p.out[nodeIdx] = o;
 }
 
-// Presence set of one item (<= 64 KiB of raw bytes): the bytes at first, first+stride, ... into local[8].
-EB_HD MaskItem mask_item_scan(const MaskParams& p, int itemIdx, int first, int stride, uint32_t (&local)[8]) {
+// Presence set of one item (<= 64 KiB of raw bytes): the bytes at first, first+stride, ... into local[8].  Strand batches
+// (p.rc): bytes of the read block are also written complemented to their place in the reverse-complement block, whose
+// presence set goes to rcLocal[8] (zero for targets).
+EB_HD MaskItem mask_item_scan(const MaskParams& p, int itemIdx, int first, int stride, uint32_t (&local)[8], uint32_t (&rcLocal)[8]) {
     MaskItem it;
     if (itemIdx < p.numItems) {
         it = p.items[itemIdx];
     } else {
         const int q = itemIdx - p.numItems;
-        it.off = p.qoff[q];
-        it.len = p.qlen[q] <= 65536 ? p.qlen[q] : 0;
-        it.dst = q;
+        const int pair = p.rc ? 2 * q : q;
+        it.off = p.qoff[pair];
+        it.len = p.qlen[pair] <= 65536 ? p.qlen[pair] : 0;
+        it.dst = pair;
     }
-    for (int k = 0; k < 8; ++k) local[k] = 0;
+    for (int k = 0; k < 8; ++k) local[k] = rcLocal[k] = 0;
     const uint8_t* s = p.raw + it.off;
+    const bool rc = p.rc && it.off < p.rcBytes;
     for (int i = first; i < it.len; i += stride) {
         const uint32_t b = s[i];
         local[b >> 5] |= 1u << (b & 31);
+        if (rc) {
+            const uint32_t c = complement_byte((uint8_t)b);
+            p.rc[p.rcBytes - 1 - (it.off + (uint64_t)i)] = (uint8_t)c;
+            rcLocal[c >> 5] |= 1u << (c & 31);
+        }
     }
     return it;
 }
@@ -1881,9 +1952,10 @@ EB_HD void mask_item_commit(const MaskParams& p, int dst, int k, uint32_t bits) 
 }
 // Whole item by one caller (host emulation).
 EB_HD void mask_item(const MaskParams& p, int itemIdx, int first, int stride) {
-    uint32_t local[8];
-    const MaskItem it = mask_item_scan(p, itemIdx, first, stride, local);
+    uint32_t local[8], rcLocal[8];
+    const MaskItem it = mask_item_scan(p, itemIdx, first, stride, local, rcLocal);
     for (int k = 0; k < 8; ++k) mask_item_commit(p, it.dst, k, local[k]);
+    for (int k = 0; k < 8; ++k) mask_item_commit(p, it.dst + 1, k, rcLocal[k]);  // (nothing for targets and plain batches)
 }
 
 // Presence set of query `q` of a QAlphaParams run: the bytes at first, first+stride, ... into local[8].

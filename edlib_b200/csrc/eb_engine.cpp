@@ -151,8 +151,10 @@ Prepared* Engine::prepare(const BatchInput& in) {
         p->alnPool.clear();
         p->N = in.numPairs;
         p->cfg = in.config;
+        p->strands = in.strands;
+        p->strand.clear();
         p->mode = (in.config.mode == EDLIB_MODE_SHW) ? MODE_SHW : (in.config.mode == EDLIB_MODE_HW) ? MODE_HW : MODE_NW;
-        const int N = p->N;
+        int N = p->N;  // the caller's pairs; a strand batch doubles it after packing
         p->qlen.resize(N);
         p->tlen.resize(N);
         p->tidx.resize(N);
@@ -234,26 +236,31 @@ Prepared* Engine::prepare(const BatchInput& in) {
 
         // pack: queries back to back, then every target 16-aligned with >= 16 bytes of slack
         size_t total = 0;
-        std::vector<int> longQueries;  // beyond one presence-set work item
         for (int i = 0; i < N; ++i) {
             p->qoff[i] = total;
             total += (size_t)p->qlen[i];
-            if (p->qlen[i] > 65536) longQueries.push_back(i);
         }
+        const size_t readBytes = total;
         total = round_up(total, 16);
         for (int t = 0; t < T; ++t) {
             p->tg[t].off = total;
             total += round_up((size_t)p->tg[t].len, 16) + 16;
         }
         total += 16;
+        // strand batches: the reverse complements of the reads follow on the device only (written there, never uploaded)
+        const size_t rcBase = total;
+        const size_t devTotal = in.strands ? rcBase + round_up(readBytes, 16) + 16 : total;
         HostBuf<uint8_t> stageBuf(be, total);  // released on every path out of this function
         uint8_t* stage = stageBuf.p;
-        p->dSeq.alloc(be, total);
+        p->dSeq.alloc(be, devTotal);
         // the small per-pair arrays go first: they would otherwise queue behind the sequences
-        p->dQoff.alloc(be, N);
-        p->dQoff.upload(p->qoff.data(), N);
-        p->dQlen.alloc(be, N);
-        p->dQlen.upload(p->qlen.data(), N);
+        auto upload_pair_arrays = [&]() {
+            p->dQoff.alloc(be, N);
+            p->dQoff.upload(p->qoff.data(), N);
+            p->dQlen.alloc(be, N);
+            p->dQlen.upload(p->qlen.data(), N);
+        };
+        if (!in.strands) upload_pair_arrays();
         trace.mark("prepare: offsets + buffers");
         {
             // Pure memcpy work, split by bytes over a few host threads when the batch is large: items
@@ -333,6 +340,32 @@ Prepared* Engine::prepare(const BatchInput& in) {
         }
         trace.mark("prepare: pack");
         stats.h2dBytes += (long long)total;
+        if (in.strands) {
+            // read i becomes pairs 2i (as uploaded) and 2i+1: its reverse complement, which the presence-set pass writes
+            // into the region at rcBase on raw bytes, before alphabet lengths and codes are derived
+            const int R = N;
+            N = p->N = 2 * R;
+            p->qlen.resize(N);
+            p->tlen.resize(N);
+            p->tidx.resize(N);
+            p->qoff.resize(N);
+            for (int i = R - 1; i >= 0; --i) {
+                const int m = p->qlen[i], n = p->tlen[i], t = p->tidx[i];
+                const uint64_t off = p->qoff[i];
+                p->qlen[2 * i] = p->qlen[2 * i + 1] = m;
+                p->tlen[2 * i] = p->tlen[2 * i + 1] = n;
+                p->tidx[2 * i] = p->tidx[2 * i + 1] = t;
+                p->qoff[2 * i] = off;
+                p->qoff[2 * i + 1] = rcBase + (readBytes - off - (uint64_t)m);  // the region is the reversed read block
+            }
+            upload_pair_arrays();
+            be->zero(p->dSeq.p + rcBase + readBytes, devTotal - rcBase - readBytes);
+        }
+        // the presence-set pass writes the reverse complements (MaskParams::rc): only the reads as given are work items
+        const int qstep = in.strands ? 2 : 1;
+        std::vector<int> longQueries;  // beyond one presence-set work item
+        for (int i = 0; i < N; i += qstep)
+            if (p->qlen[i] > 65536) longQueries.push_back(i);
 
         // byte-presence sets: one per query, one per distinct target, one union for the batch.  Queries are
         // implicit work items of the kernel; explicit ones (at most 65536 bytes each) are only needed for
@@ -360,9 +393,13 @@ Prepared* Engine::prepare(const BatchInput& in) {
             mp.numItems = (int)items.size();
             mp.qoff = p->dQoff.p;
             mp.qlen = p->dQlen.p;
-            mp.numQueries = N;
+            mp.numQueries = N / qstep;
             mp.masks = dMasks.p;
             mp.unionSet = unionSet;
+            if (in.strands) {
+                mp.rc = p->dSeq.p + rcBase;
+                mp.rcBytes = (uint64_t)readBytes;
+            }
             if (mp.numItems + mp.numQueries > 0) be->launch_mask(mp);
         }
         DevBuf<int> dTset(be, N), dAlpha(be, N);
@@ -440,7 +477,7 @@ Prepared* Engine::prepare(const BatchInput& in) {
         }
         DevBuf<uint8_t> dMap(be, 256);
         dMap.upload(map, 256);
-        EncodeParams ep{p->dSeq.p, (uint64_t)total, dMap.p};
+        EncodeParams ep{p->dSeq.p, (uint64_t)devTotal, dMap.p};
         be->launch_encode(ep);
         if (anyEq) {
             p->dEqtab.alloc(be, eq.size());
@@ -569,6 +606,8 @@ void Engine::compute(Prepared* p) {
     std::vector<Route> routes;
     long long devReads = 0, devListed = 0;
     int devSlices = 0;
+    // a group list of a strand batch holds the two strands of a read next to each other: even slices keep them together
+    const int sliceReads = p->strands ? tun.devSliceReads & ~1 : tun.devSliceReads;
     for (auto& kv : groups) {
         const std::vector<int>& list = kv.second;
         // Small groups go to the warp kernel, except HW over a long target: there the lane kernel
@@ -590,7 +629,7 @@ void Engine::compute(Prepared* p) {
         routes.push_back(Route{t, nw, &list, dev});
         if (dev) {
             devReads += (long long)list.size();
-            devSlices += ceil_div((int)list.size(), tun.devSliceReads);
+            devSlices += ceil_div((int)list.size(), sliceReads);
             const bool consecutive = (long long)list.back() - list.front() + 1 == (long long)list.size();
             if (!consecutive) devListed += (long long)list.size();
         }
@@ -616,9 +655,9 @@ void Engine::compute(Prepared* p) {
                 rows.fetch_add(s, std::memory_order_relaxed);
             });
             stats.k1Cells += rows.load() * (long long)p->tg[r.t].len;
-            for (int first = 0; first < (int)list.size(); first += tun.devSliceReads)
+            for (int first = 0; first < (int)list.size(); first += sliceReads)
                 ps.dev_enqueue_slice(r.t, r.nw, consecutive ? list.front() : -1, list.data(), first,
-                                     std::min(tun.devSliceReads, (int)list.size() - first));
+                                     std::min(sliceReads, (int)list.size() - first));
         }
         p->endPool.resize((size_t)ps.poolReserved);  // what the slices were actually handed
         trace.mark("compute: device stage enqueued");
@@ -646,6 +685,7 @@ void Engine::compute(Prepared* p) {
     } else {
         ps.collect_ends(nullptr);
     }
+    if (p->strands) ps.pick_strands();
     trace.mark("compute: end locations");
     ps.start_locations();
     ps.paths();
@@ -735,11 +775,13 @@ static void free_result_arrays(EdlibAlignResult* results, int n) {
 void Engine::materialize(Prepared* p, EdlibAlignResult* results) {
     if (!p->computed) throw std::runtime_error("results requested from a batch that was not (successfully) computed");
     Trace trace;
-    const int N = p->N;
+    const int N = p->strands ? p->N / 2 : p->N;  // a strand batch: one result per read, from its winning strand
     std::atomic<int> failed(0);
     parallel_ranges((size_t)N, 65536, [&](size_t lo, size_t hi) {
-        for (int i = (int)lo; i < (int)hi; ++i)
-            if (!materialize_one(p, i, results[i])) failed.store(1, std::memory_order_relaxed);
+        for (int i = (int)lo; i < (int)hi; ++i) {
+            const int pair = p->strands ? 2 * i + p->strand[i] : i;
+            if (!materialize_one(p, pair, results[i])) failed.store(1, std::memory_order_relaxed);
+        }
     });
     if (failed.load()) {
         free_result_arrays(results, N);
@@ -840,7 +882,13 @@ void Engine::target_free(TargetHandle* h) {
         }
 }
 
-int Engine::align_batch(const BatchInput& in, EdlibAlignResult* results) {
+void Engine::strands_of(const Prepared* p, unsigned char* strands) const {
+    if (!p->strands) throw std::runtime_error("strands requested from a batch not prepared with strands");
+    if (!p->computed) throw std::runtime_error("strands requested from a batch that was not (successfully) computed");
+    memcpy(strands, p->strand.data(), p->strand.size());
+}
+
+int Engine::align_batch(const BatchInput& in, EdlibAlignResult* results, unsigned char* strands) {
     Prepared* p = nullptr;
     stats = EngineStats();
     statsPending_ = false;
@@ -851,6 +899,7 @@ int Engine::align_batch(const BatchInput& in, EdlibAlignResult* results) {
         compute(p);
         built = true;
         materialize(p, results);  // releases what it built when it fails
+        if (strands) strands_of(p, strands);
         release(p);
         return EDLIB_STATUS_OK;
     } catch (const std::exception& e) {
@@ -907,7 +956,7 @@ struct StreamJob {
 bool Engine::align_streamed(const BatchInput& in, EdlibAlignResult* results) {
     Backend* be = be_;
     const int N = in.numPairs;
-    if (in.config.mode != EDLIB_MODE_HW || N < tun.streamMinPairs || !tun.deviceStage) return false;
+    if (in.config.mode != EDLIB_MODE_HW || N < tun.streamMinPairs || !tun.deviceStage || in.strands) return false;
     if (in.config.additionalEqualities && in.config.additionalEqualitiesLength > 0) return false;
     if (tun.filterSeedK <= 0 || tun.filterSeedLevels <= 0) return false;
     const char* tptr = in.targets[0];
@@ -964,6 +1013,7 @@ bool Engine::align_streamed(const BatchInput& in, EdlibAlignResult* results) {
         p->otherPairs.clear();
         p->N = N;
         p->cfg = in.config;
+        p->strands = false;
         p->mode = MODE_HW;
         p->qlen.resize(N);
         p->tlen.resize(N);

@@ -97,6 +97,7 @@ struct BatchInput {
     const int* targetLengths;
     int numPairs;
     EdlibAlignConfig config;
+    bool strands = false;  // align every query and its reverse complement, report the better strand (Prepared::strands)
 };
 
 struct EngineTunables {
@@ -168,8 +169,10 @@ class Engine {
 public:
     explicit Engine(Backend* be);
     ~Engine();
-    // One-shot: prepare + compute + materialise.  Returns EDLIB_STATUS_OK / EDLIB_STATUS_ERROR.
-    int align_batch(const BatchInput& in, EdlibAlignResult* results);
+    // One-shot: prepare + compute + materialise (and, for a strand batch, the chosen strand per read into `strands`).
+    // Returns EDLIB_STATUS_OK / EDLIB_STATUS_ERROR.
+    int align_batch(const BatchInput& in, EdlibAlignResult* results, unsigned char* strands = nullptr);
+    void strands_of(const Prepared* p, unsigned char* strands) const;  // a computed strand batch: 1 where the reverse strand won
 
     // Staged form (bench "inputs resident in HBM" measurement, multi-GPU shards):
     Prepared* prepare(const BatchInput& in);                 // upload, alphabet, encode

@@ -333,6 +333,10 @@ class Prepared {
 public:
     Backend* be = nullptr;
     int N = 0;
+    // Strand batch: read i of the caller is pair 2i (as given) and pair 2i+1 (its reverse complement, written by the
+    // presence-set pass into a second query region); N counts both.  `strand` is the chosen strand per read (Pass::pick_strands).
+    bool strands = false;
+    std::vector<uint8_t> strand;
     EdlibAlignConfig cfg{};
     int mode = MODE_NW;  // normalised: anything that is not SHW/HW runs as NW (ref cpp:205-215)
     std::vector<int> qlen, tlen, tidx;
@@ -686,6 +690,16 @@ struct Pass {
     // read moves on to `next`.
     void no_distance_within(LaneGroup& c, int s, int t, std::vector<int>& next);
 
+    // Strand batches: the cross-strand rule (eb_core.h: strand_rule) over the reads of `list` whose other strand is in
+    // the list as well (at s + 1 for a forward pair s).  The reads of the `pending` lists are undecided (excl / bound
+    // per read), the others decided (best[]).  Tightens the bounds; a losing pending read is decided as "no alignment"
+    // and leaves its list.
+    void strand_prune(const std::vector<int>& list, const std::vector<int>& excl, std::vector<int>& bound,
+                      std::initializer_list<std::vector<int>*> pending);
+    // After the end locations: per read of a strand batch, the winning strand (Prepared::strand); the loser's result
+    // becomes "no alignment", so that start locations and paths are only computed for winners.
+    void pick_strands();
+
     // Seed stage, host-driven: exact seeds of every read looked up in the index of the target; windows around
     // the expected end columns are planned, swept and reduced on the device (eb_core.h: seed_plan_read), the
     // outcome per read is worked out on the host.
@@ -706,8 +720,9 @@ struct Pass {
     // rows), host-driven: the stages of the candidate filter (HW over a long target; DESIGN.md section 5), each on
     // the reads the previous ones left undecided, then the plain lane-per-alignment sweep of what is left.
     // `excl` (or nullptr) carries what the device-driven first level found out about the reads (-2: plain sweep),
-    // `firstSeedLevel` the first seed level still to try.
-    void lane_group(int t, int nw, const std::vector<int>& list, const std::vector<int>* excl = nullptr, int firstSeedLevel = 0);
+    // `bounds` their bounds, `firstSeedLevel` the first seed level still to try.
+    void lane_group(int t, int nw, const std::vector<int>& list, const std::vector<int>* excl = nullptr,
+                    const std::vector<int>* bounds = nullptr, int firstSeedLevel = 0);
 
     // ---- device-driven first seed level ----------------------------------------------------------------
     // May group (t, nw) take it?  (HW over a long target, plain equality, seed stage enabled, index available.)

@@ -570,15 +570,22 @@ __global__ void mask_kernel(const MaskParams p) {
     const int item = blockIdx.x * W_WARPS + (threadIdx.x >> 5);
     if (item >= p.numItems + p.numQueries) return;
     // lanes stride over the bytes; the eight words are OR-reduced across the warp and lane k commits word k
-    uint32_t local[8];
-    const MaskItem it = mask_item_scan(p, item, threadIdx.x & 31, 32, local);
-    uint32_t mine = 0;
+    uint32_t local[8], rcLocal[8];
+    const MaskItem it = mask_item_scan(p, item, threadIdx.x & 31, 32, local, rcLocal);
+    uint32_t mine = 0, rcMine = 0;
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
         const uint32_t v = __reduce_or_sync(0xffffffffu, local[k]);
-        if ((int)(threadIdx.x & 31) == k) mine = v;
+        const uint32_t w = __reduce_or_sync(0xffffffffu, rcLocal[k]);
+        if ((int)(threadIdx.x & 31) == k) {
+            mine = v;
+            rcMine = w;
+        }
     }
-    if ((threadIdx.x & 31) < 8) mask_item_commit(p, it.dst, (int)(threadIdx.x & 31), mine);
+    if ((threadIdx.x & 31) < 8) {
+        mask_item_commit(p, it.dst, (int)(threadIdx.x & 31), mine);
+        mask_item_commit(p, it.dst + 1, (int)(threadIdx.x & 31), rcMine);  // strand batches: the reverse complement's set
+    }
 }
 
 __global__ void alpha_len_kernel(const uint32_t* masks, const int* qset, const int* tset, int n, int* out) {

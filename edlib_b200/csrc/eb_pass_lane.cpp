@@ -353,6 +353,39 @@ void Pass::no_distance_within(LaneGroup& c, int s, int t, std::vector<int>& next
     }
 }
 
+void Pass::strand_prune(const std::vector<int>& list, const std::vector<int>& excl, std::vector<int>& bound,
+                        std::initializer_list<std::vector<int>*> pending) {
+    const int G = (int)list.size();
+    std::vector<uint8_t> state(G, 0);  // 0 decided, 1 pending, 2 lost here
+    for (std::vector<int>* v : pending)
+        for (int s : *v) state[s] = 1;
+    bool lost = false;
+    for (int s = 0; s + 1 < G; ++s) {
+        if ((list[s] & 1) || list[s + 1] != list[s] + 1) continue;
+        bool done[2];
+        int d[2], ex[2], bd[2];
+        for (int h = 0; h < 2; ++h) {
+            done[h] = state[s + h] == 0;
+            d[h] = done[h] ? best[list[s + h]] : 0x7fffffff;
+            ex[h] = excl[s + h];
+            bd[h] = bound[s + h];
+        }
+        const int loser = strand_rule(done, d, ex, bd);
+        bound[s] = bd[0];
+        bound[s + 1] = bd[1];
+        if (loser < 0) continue;
+        const int pair = list[s + loser];
+        best[pair] = 0x7fffffff;
+        cnt[pair] = 0;
+        posLen[pair] = 0;
+        state[s + loser] = 2;
+        stats.filterDecided++;
+        lost = true;
+    }
+    if (!lost) return;
+    for (std::vector<int>* v : pending) v->erase(std::remove_if(v->begin(), v->end(), [&](int s) { return state[s] == 2; }), v->end());
+}
+
 // Seed stage, host-driven: exact seeds of every read looked up in the index of the target; windows around
 // the expected end columns are planned, swept and reduced on the device (eb_core.h: seed_plan_read).
 void Pass::seed_stage(LaneGroup& c, int level, const std::vector<int>& in, std::vector<int>& next) {
@@ -377,7 +410,7 @@ void Pass::seed_stage(LaneGroup& c, int level, const std::vector<int>& in, std::
         for (size_t i = lo; i < hi; ++i) {
             const int s = cand[i];
             rl[i] = list[s];
-            hThr[i] = seed_threshold(p->qlen[list[s]], k, L, tun.filterSeedK, excl[s]);
+            hThr[i] = seed_threshold(p->qlen[list[s]], bound[s], L, tun.filterSeedK, excl[s]);
         }
     });
     DevBuf<int> dList(be, g), dThr(be, g), dCount(be, 1);
@@ -737,7 +770,8 @@ void Pass::plain_sweep(LaneGroup& c) {
 // Distance pass of one group of pairs that share target `t` and word class `nw` (queries <= 256
 // rows), host-driven: the stages of the candidate filter (HW over a long target; DESIGN.md section 5), each on the
 // reads the previous ones left undecided, then the plain lane-per-alignment sweep of what is left.
-void Pass::lane_group(int t, int nw, const std::vector<int>& list, const std::vector<int>* exclInit, int firstSeedLevel) {
+void Pass::lane_group(int t, int nw, const std::vector<int>& list, const std::vector<int>* exclInit, const std::vector<int>* boundInit,
+                      int firstSeedLevel) {
     const Target& tg = p->tg[t];
     const int G = (int)list.size();
     LaneGroup c{t, nw, list, tg, tg.len, std::vector<int>(G), std::vector<int>(G, -1), std::vector<int>(), std::vector<uint8_t>(G, 0)};
@@ -745,7 +779,7 @@ void Pass::lane_group(int t, int nw, const std::vector<int>& list, const std::ve
     long long rows = 0;
     for (int s = 0; s < G; ++s) {
         const int m = p->qlen[list[s]];
-        c.bound[s] = (k < 0 || k > m) ? m : k;  // distances never exceed m in HW/SHW (ref cpp:566-568)
+        c.bound[s] = boundInit ? (*boundInit)[s] : (k < 0 || k > m) ? m : k;  // distances never exceed m in HW/SHW (ref cpp:566-568)
         rows += m;
     }
     if (!exclInit) stats.k1Cells += rows * (long long)c.n;  // (device-driven groups were counted when enqueued)
@@ -770,6 +804,7 @@ void Pass::lane_group(int t, int nw, const std::vector<int>& list, const std::ve
             std::vector<int> next;
             seed_stage(c, level, cur, next);
             cur.swap(next);
+            if (p->strands) strand_prune(list, c.excl, c.bound, {&cur, &c.direct});
         }
         // Reads that drowned in seed occurrences at the last level tried are repeats: their prefixes match all over
         // the target as well, so the prefix stages would cost two more sweeps and decide few of them.
@@ -786,6 +821,7 @@ void Pass::lane_group(int t, int nw, const std::vector<int>& list, const std::ve
             std::vector<int> next;
             prefix_stage(c, stageP[st], stageK[st], cur, next);
             cur.swap(next);
+            if (p->strands) strand_prune(list, c.excl, c.bound, {&cur, &c.direct});
         }
     }
     if (trace.on)
@@ -876,6 +912,7 @@ int Pass::dev_enqueue_slice(int t, int nw, int firstPair, const int* listHost, i
     rp.firstPair = sl.firstPair;
     rp.qlen = p->dQlen.p;
     rp.kBound = k;
+    rp.strands = p->strands;
     reduce_windows(rp, dPlan.p, count, wr, dOut.p, dExtra.p, dCtr.p + 1, extraCap);
     FinParams fp;
     memset(&fp, 0, sizeof(fp));
@@ -895,6 +932,11 @@ int Pass::dev_enqueue_slice(int t, int nw, int firstPair, const int* listHost, i
     fp.poolCap = sl.poolCap;
     fp.header = dHeaders.p + 4 * si;
     fp.winCount = dCtr.p;
+    if (p->strands) {  // the slice holds both strands of its reads (even offsets into a group list of pair couples)
+        fp.strands = 1;
+        fp.leftover = dLeft.p;
+        fp.leftoverCount = dLeftCount.p;
+    }
     be->launch_fin_count(fp);
     be->launch_scan(dCnt32.p, count);
     be->launch_fin_fill(fp);
@@ -958,20 +1000,24 @@ void Pass::dev_leftovers() {
     HostBuf<Leftover> left(be, (size_t)std::max(L, 1));
     if (L) be->d2h(left.p, dLeft.p, (size_t)L * sizeof(Leftover));
     else be->sync();
-    stats.d2hBytes += 4 + 8LL * L;
+    stats.d2hBytes += 4 + (long long)sizeof(Leftover) * L;
     trace.mark("device stage: results on the host");
     if (L == 0) return;
     std::sort(left.p, left.p + L, [](const Leftover& a, const Leftover& b) { return a.pair < b.pair; });
     trace.mark("device stage: leftovers sorted");
-    std::map<std::pair<int, int>, std::pair<std::vector<int>, std::vector<int>>> groups;  // (t, nw) -> pairs, excl
+    struct Group {
+        std::vector<int> pairs, excl, bound;
+    };
+    std::map<std::pair<int, int>, Group> groups;  // (t, nw) -> reads
     for (int i = 0; i < L; ++i) {
         const int pair = left[i].pair;
-        auto& g = groups[std::make_pair(p->tidx[pair], ceil_div(p->qlen[pair], 32))];
-        g.first.push_back(pair);
-        g.second.push_back(left[i].excl);
+        Group& g = groups[std::make_pair(p->tidx[pair], ceil_div(p->qlen[pair], 32))];
+        g.pairs.push_back(pair);
+        g.excl.push_back(left[i].excl);
+        g.bound.push_back(left[i].bound);
         hostPairs.push_back(pair);
     }
     trace.mark("device stage: leftovers grouped");
-    for (auto& kv : groups) lane_group(kv.first.first, kv.first.second, kv.second.first, &kv.second.second, 1);
+    for (auto& kv : groups) lane_group(kv.first.first, kv.first.second, kv.second.pairs, &kv.second.excl, &kv.second.bound, 1);
 }
 }  // namespace eb

@@ -153,6 +153,8 @@ void Pass::long_hw_distance(const std::vector<int>& pairs) {
                     rest.push_back(s);
                 }
             }
+            // the losing strand of a read never reaches the chunked sweep of the whole target
+            if (p->strands) strand_prune(list, excl, bound, {&cur, &rest});
         }
         cur.swap(rest);
         std::sort(cur.begin(), cur.end());
@@ -348,6 +350,25 @@ void Pass::collect_ends(const std::vector<int>* pairs) {
             if (a > posLen[i]) p->endPool[(size_t)at++] = -1;
             if (posLen[i]) memcpy(p->endPool.data() + at, posPool.data() + posStart[i], sizeof(int) * (size_t)posLen[i]);
             at += posLen[i];
+        }
+    });
+}
+
+// Every route (device-driven level, host-driven stages, warp and band kernels, NW / SHW, equalities) has left the exact
+// distance of each strand within its bound; the reverse strand wins when it has a distance and the forward strand a
+// larger one or none.  Ties and "neither within k" report the forward strand.
+void Pass::pick_strands() {
+    const int R = N / 2;
+    p->strand.assign((size_t)R, 0);
+    parallel_ranges((size_t)R, 65536, [&](size_t lo, size_t hi) {
+        for (size_t i = lo; i < hi; ++i) {
+            const int f = 2 * (int)i, r = f + 1;
+            if (p->special[f]) continue;  // an empty sequence: both strands give the same result
+            const bool rev = p->ed[r] >= 0 && (p->ed[f] < 0 || p->ed[r] < p->ed[f]);
+            const int loser = rev ? f : r;
+            p->strand[i] = rev ? 1 : 0;
+            p->ed[loser] = -1;
+            p->endCount[loser] = 0;
         }
     });
 }

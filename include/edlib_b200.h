@@ -70,6 +70,27 @@ EDLIB_API int edlibB200BatchCompute(EdlibB200Batch* batch, EdlibB200Stats* stats
 EDLIB_API int edlibB200BatchResults(EdlibB200Batch* batch, EdlibAlignResult* results);
 EDLIB_API void edlibB200BatchFree(EdlibB200Batch* batch);
 
+/* Both strands of DNA reads in one call.  For each pair i, queries[i] and its reverse complement rc(queries[i]) are
+ * aligned to targets[i]: rc reverses the query and complements every byte with a fixed table (A<->T, C<->G, R<->Y,
+ * K<->M, B<->V, D<->H, upper and lower case; every other byte, N / S / W and non-letters included, is its own
+ * complement).  results[i] is the result of edlibAlign(rc(queries[i]), targets[i], config), with strands[i] = 1, when
+ * that one has a distance and the forward one has a larger distance or none; otherwise it is the result of
+ * edlibAlign(queries[i], targets[i], config), with strands[i] = 0 -- ties and "neither strand within k" report the
+ * forward strand.  Every field is that of the chosen strand (the alignment of the reverse strand is that of
+ * rc(queries[i])).  Any mode, task, k and additional equalities; for HW read sets over a long target, the distance the
+ * seed filter finds on one strand bounds the search on the other.  Returns EDLIB_STATUS_OK / EDLIB_STATUS_ERROR. */
+EDLIB_API int edlibB200AlignBatchStrands(const char* const* queries, const int* queryLengths,
+                                         const char* const* targets, const int* targetLengths, int numPairs,
+                                         const EdlibAlignConfig config, EdlibAlignResult* results, unsigned char* strands);
+/* Staged form of edlibB200AlignBatchStrands: the reads are uploaded once, their reverse complements are made on the
+ * device.  edlibB200BatchCompute / edlibB200BatchResults then work as for any batch and give numPairs results. */
+EDLIB_API EdlibB200Batch* edlibB200BatchPrepareStrands(const char* const* queries, const int* queryLengths,
+                                                       const char* const* targets, const int* targetLengths,
+                                                       int numPairs, const EdlibAlignConfig config);
+/* strands[i] (numPairs bytes) of the last edlibB200BatchCompute of a strand batch; EDLIB_STATUS_ERROR for a batch not
+ * prepared with edlibB200BatchPrepareStrands, or one that was not computed. */
+EDLIB_API int edlibB200BatchStrands(EdlibB200Batch* batch, unsigned char* strands);
+
 /* A target kept resident on the device.  edlibAlignBatch calls of read sets (HW, short queries, plain equality) whose
  * targets[i] all equal (target, targetLength) of a live handle skip the target's upload, its encoding and the build of
  * its seed index: a caller that aligns many batches to one genome pays them once.  The bytes at `target` must not
