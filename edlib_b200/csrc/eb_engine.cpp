@@ -109,7 +109,6 @@ EngineTunables::EngineTunables() {
     const int sliceMb = env_int("EDLIB_B200_SLICE_MB", 0);
     if (sliceMb > 0) sliceBytes = (size_t)sliceMb << 20;
     if (sliceMb > 0) pathSliceBytes = (size_t)sliceMb << 20;
-    deviceResults = env_int("EDLIB_B200_DEVICE_RESULTS", deviceResults);
 }
 
 // dense codes in ascending byte order for the bytes of `present`; every other byte maps to `other`

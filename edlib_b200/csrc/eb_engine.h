@@ -106,7 +106,6 @@ struct EngineTunables {
     int ovfCap = 1 << 20;         // overflow entries per launch before the exact-size retry
     size_t sliceBytes = 1ull << 30;  // device memory budget of one slice of W jobs
     size_t pathSliceBytes = 8ull << 30;  // ... of one slice of device-driven paths of short queries (stored matrices)
-    int deviceResults = 1;        // start locations / paths of short queries driven from the device (0: per-job host objects)
     size_t packParallelBytes = 32u << 20;  // batches above this are packed and uploaded by several host threads
     // Candidate filter for HW sweeps of reads over a shared target, three stages (0 disables one):
     // exact seeds looked up in a hash index of the target (pigeonhole: t+1 disjoint seeds for threshold

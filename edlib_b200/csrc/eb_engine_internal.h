@@ -394,8 +394,12 @@ struct WRunner {
     Backend* be;
     Prepared* p;
     std::vector<uint8_t>* opsPool = nullptr;
+    int laneOk[9] = {-1, -1, -1, -1, -1, -1, -1, -1, -1};
 
     size_t task_bytes(const WTask& t) const;
+
+    // Can the lane kernels sweep queries of nw 32-bit words (1..8) over this batch's alphabet (Peq rows per thread)?
+    bool lane_ok(int nw);
 
     // Tasks whose query fits 256 rows and whose shape one of the lane-kernel classes covers run one
     // alignment per THREAD (lane_kernel); everything else one alignment per warp (w_kernel).
@@ -423,6 +427,11 @@ struct WRunner {
     // ovfCap == 0: first pass (no position list).  ovfCap > 0: second pass over the tasks whose
     // end-location lists exceed KPOS, started from their known minimum with an exact-size list.
     void run_slice(std::vector<WTask>& tasks, const std::vector<int>& slice, int R, int ovfCap);
+
+    // Traceback of the matrix-storing sweeps just launched over `mat`: tb[i] belongs to tasks[owner[i]], whose edit script
+    // is appended to the ops pool.  `peq`: the warp kernel's Peq rows, or nullptr with TbJob::peqOff = ~0 (lane kernel).
+    void traceback(std::vector<WTask>& tasks, const std::vector<TbJob>& tb, const std::vector<int>& owner, const U2* mat,
+                   const uint32_t* peq);
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -514,7 +523,6 @@ struct Pass {
     std::vector<int> wPairs;          // pairs swept by the warp / lane-job kernels
     std::vector<uint8_t> opsPool;
     WRunner runner;
-    int laneOkCache[9] = {-1, -1, -1, -1, -1, -1, -1, -1, -1};
 
     // ---- device-driven first seed level (eb_pass_lane.cpp) ----
     bool devMode = false;             // some group of this pass runs it: results are assembled per slice on the device
@@ -565,76 +573,6 @@ struct Pass {
                 posLen[i] = 0;
             }
         });
-    }
-
-    // ---- direct lane-kernel launches (no per-job host objects): the LOC / PATH phases of large read
-    // batches issue millions of tiny sweeps, so their jobs are built straight into LJob arrays. --------
-    bool lane_ok(int m);
-
-    void lane_launch(const std::vector<LJob>& jobs, int nw, int laneMode, bool rev, std::vector<Rec>& recs);
-
-    // Matrix-storing NW sweeps + traceback of `jobs` (matOff is assigned here); `sink(jobIndex, ops, len,
-    // score)` receives every edit script.  Slices bound the stored matrices to the slice budget.
-    template <class Sink>
-    void lane_paths(std::vector<LJob>& jobs, int nw, Sink sink) {
-        size_t a = 0;
-        while (a < jobs.size()) {
-            size_t bytes = 0, b = a;
-            uint64_t matEntries = 0, opsBytes = 0;
-            std::vector<TbJob> tb;
-            while (b < jobs.size()) {
-                LJob& j = jobs[b];
-                const size_t need = (size_t)j.n * nw * 8 + (size_t)j.m + j.n + sizeof(LJob) + sizeof(TbJob) + 64;
-                if (b > a && bytes + need > tun.sliceBytes) break;
-                j.matOff = matEntries;
-                TbJob t;
-                memset(&t, 0, sizeof(t));
-                t.matOff = matEntries;
-                t.qOff = j.qOff;
-                t.peqOff = ~0ull;
-                t.tOff = j.tOff;
-                t.outOff = opsBytes;
-                t.m = j.m;
-                t.n = j.n;
-                t.nWp = nw;
-                tb.push_back(t);
-                matEntries += (uint64_t)j.n * nw;
-                opsBytes += (uint64_t)j.m + j.n;
-                bytes += need;
-                ++b;
-            }
-            const size_t n = b - a;
-            DevBuf<LJob> dJobs(be, n);
-            dJobs.upload(jobs.data() + a, n);
-            DevBuf<Rec> dRecs(be, n);
-            be->zero(dRecs.p, n * sizeof(Rec));
-            DevBuf<U2> dMat(be, matEntries);
-            LParams lp{dJobs.p, (int)n, p->dSeq.p, p->dSeq.p, p->ncodes, p->hasEq ? p->dEqtab.p : nullptr, dRecs.p, dMat.p, 1};
-            be->launch_lane(lp, nw, MODE_NW, false, true);
-            DevBuf<TbJob> dTb(be, n);
-            dTb.upload(tb.data(), n);
-            DevBuf<uint8_t> dOps(be, opsBytes);
-            DevBuf<int> dStart(be, n), dLen(be, n);
-            TbParams tp{dTb.p, (int)n, dMat.p, nullptr, p->dSeq.p, p->dSeq.p, p->hasEq ? p->dEqtab.p : nullptr, p->ncodes,
-                        dOps.p, dStart.p, dLen.p, 1};
-            be->launch_traceback(tp);
-            // one pinned staging block for everything that comes back (fast D2H, no zero-fill of vectors)
-            const size_t offSt = round_up(n * sizeof(Rec), 64), offLn = offSt + round_up(n * sizeof(int), 64);
-            const size_t offOps = offLn + round_up(n * sizeof(int), 64);
-            HostBuf<uint8_t> hostBuf(be, offOps + opsBytes);  // released on every path out, exceptions included
-            uint8_t* host = hostBuf.p;
-            const Rec* recs = reinterpret_cast<const Rec*>(host);
-            const int* st = reinterpret_cast<const int*>(host + offSt);
-            const int* ln = reinterpret_cast<const int*>(host + offLn);
-            const uint8_t* ops = host + offOps;
-            be->d2h(host, dRecs.p, n * sizeof(Rec));
-            be->d2h(host + offSt, dStart.p, n * sizeof(int));
-            be->d2h(host + offLn, dLen.p, n * sizeof(int));
-            be->d2h(host + offOps, dOps.p, opsBytes);
-            stats.d2hBytes += (long long)opsBytes + (long long)n * (long long)(sizeof(Rec) + 8);
-            for (size_t q = 0; q < n; ++q) sink(a + q, ops + tb[q].outOff + st[q], ln[q], recs[q].best);
-            a = b;
-        }
     }
 
     // The radix seed index of the target the seed stages last worked on (one table for every level); kept in the

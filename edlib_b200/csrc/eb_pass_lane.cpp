@@ -5,36 +5,6 @@
 
 namespace eb {
 
-// ---- direct lane-kernel launches (no per-job host objects): the LOC / PATH phases of large read
-// batches issue millions of tiny sweeps, so their jobs are built straight into LJob arrays. --------
-bool Pass::lane_ok(int m) {
-    if (m <= 0 || m > 256) return false;
-    const int nw = ceil_div(m, 32);
-    if (laneOkCache[nw] < 0) {
-        int bt = 0, rc = 0;
-        be->k1_shape(nw, p->ncodes, 0x7fffffff, &bt, &rc);
-        laneOkCache[nw] = rc > 0 ? 1 : 0;
-    }
-    return laneOkCache[nw] == 1;
-}
-
-void Pass::lane_launch(const std::vector<LJob>& jobs, int nw, int laneMode, bool rev, std::vector<Rec>& recs) {
-    const size_t J = jobs.size();
-    recs.resize(J);
-    const size_t step = 4u << 20;
-    for (size_t a = 0; a < J; a += step) {
-        const size_t n = std::min(step, J - a);
-        DevBuf<LJob> dJobs(be, n);
-        dJobs.upload(jobs.data() + a, n);
-        DevBuf<Rec> dRecs(be, n);
-        be->zero(dRecs.p, n * sizeof(Rec));
-        LParams lp{dJobs.p, (int)n, p->dSeq.p, p->dSeq.p, p->ncodes, p->hasEq ? p->dEqtab.p : nullptr, dRecs.p, nullptr, 1};
-        be->launch_lane(lp, nw, laneMode, rev, false);
-        dRecs.download(recs.data() + a, n);
-        stats.d2hBytes += (long long)n * (long long)sizeof(Rec);
-    }
-}
-
 // Seed lengths and the radix index of target t (eb_common.h: SeedIndexParams).  Level 0 uses the shortest seeds
 // with sigma^L >= filterSeedSlack * n (a fraction of a chance occurrence per seed: every occurrence costs a window
 // sweep); the later levels shorter ones (more seeds fit into a read, so a higher threshold, at the price of more

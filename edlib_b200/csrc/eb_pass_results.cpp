@@ -398,8 +398,7 @@ void Pass::res_begin() {
     resClasses = 0;
     for (unsigned b : part) resClasses |= b;
     for (int nw = 1; nw <= 8; ++nw)
-        if (((resClasses >> nw) & 1u) && !lane_ok(32 * nw)) resClasses = (resClasses & ~(1u << nw)) | 1u;
-    if (!tun.deviceResults) resClasses = (resClasses & ~0x1feu) | ((resClasses & 0x1feu) ? 1u : 0u);
+        if (((resClasses >> nw) & 1u) && !runner.lane_ok(nw)) resClasses = (resClasses & ~(1u << nw)) | 1u;
     if (!(resClasses & 0x1feu)) return;
     rEd.alloc(be, (size_t)N);
     rEndCount.alloc(be, (size_t)N);
@@ -593,43 +592,21 @@ void Pass::start_locations() {
     const bool wantLoc = p->cfg.task == EDLIB_TASK_LOC || p->cfg.task == EDLIB_TASK_PATH;
     if (wantLoc) {
         p->startPool.resize(p->endPool.size());
-        if (mode != MODE_HW) {
+        if (mode == MODE_HW) start_locations_device();  // every found pair of the lane kernel's word classes (or nothing)
+        if (!(resClasses & 0x1feu))  // nothing came from the device: 0 unless a sweep below sets it (NW / SHW: every start)
             parallel_ranges(p->startPool.size(), 1 << 20, [&](size_t lo, size_t hi) { memset(p->startPool.data() + lo, 0, (hi - lo) * sizeof(int)); });
-        } else {
-            start_locations_device();  // every found pair of the lane kernel's word classes (or nothing)
-            if (!(resClasses & 0x1feu))
-                parallel_ranges(p->startPool.size(), 1 << 20, [&](size_t lo, size_t hi) { memset(p->startPool.data() + lo, 0, (hi - lo) * sizeof(int)); });
-        }
-        if (mode == MODE_HW && (resClasses & 1u)) {  // found pairs outside those classes: per-job objects on the host
+        if (mode == MODE_HW && (resClasses & 1u)) {  // found pairs outside those classes (long queries, large alphabets)
             std::vector<WTask> tasks;
             std::vector<long long> slotOf;
-            std::vector<LJob> lj[9];          // short queries: straight to the lane kernel, per word class
-            std::vector<long long> lslot[9];
-            std::vector<int> lpair[9];
             for (int i = 0; i < N; ++i) {
                 if (p->ed[i] < 0) continue;
                 const int m = p->qlen[i];
                 if (res_class(m)) continue;  // done on the device
-                const bool lane = lane_ok(m);
                 for (int q = 0; q < p->endCount[i]; ++q) {
                     p->startPool[(size_t)(p->endStart[i] + q)] = 0;
                     const long long slot = p->endStart[i] + q;
                     const int e = p->endPool[(size_t)slot];
                     if (e < 0) continue;  // ref cpp:237-249: start 0
-                    if (lane) {
-                        const int nw = ceil_div(m, 32);
-                        LJob j;
-                        memset(&j, 0, sizeof(j));
-                        j.qOff = p->qoff[i];
-                        j.tOff = p->tg[p->tidx[i]].off + (uint64_t)e;  // first symbol read, walking backward
-                        j.m = m;
-                        j.n = (int)std::min<long long>((long long)e + 1, (long long)m + p->ed[i]);
-                        j.kInit = p->ed[i] + 1;
-                        lj[nw].push_back(j);
-                        lslot[nw].push_back(slot);
-                        lpair[nw].push_back(i);
-                        continue;
-                    }
                     WTask t;
                     t.pair = i;
                     t.qOff = p->qoff[i];
@@ -654,18 +631,6 @@ void Pass::start_locations() {
                 }
             }
             trace.mark("starts: jobs built");
-            for (int nw = 1; nw <= 8; ++nw) {
-                if (lj[nw].empty()) continue;
-                std::vector<Rec> recs;
-                lane_launch(lj[nw], nw, MODE_SHW, true, recs);
-                for (size_t j = 0; j < recs.size(); ++j) {
-                    if (recs[j].cnt <= 0 || recs[j].best != p->ed[lpair[nw][j]])
-                        throw std::runtime_error("internal: start-location sweep disagrees");
-                    const int e = p->endPool[(size_t)lslot[nw][j]];
-                    p->startPool[(size_t)lslot[nw][j]] = e - recs[j].last;  // ref cpp:260
-                }
-            }
-            trace.mark("starts: lane sweeps");
             runner.run(tasks);
             for (size_t j = 0; j < tasks.size(); ++j) {
                 const WTask& t = tasks[j];
@@ -797,22 +762,8 @@ void Pass::paths() {
         }
         {
             std::vector<WTask> tasks;
-            std::vector<LJob> lj[9];  // leaves with short queries: lane kernel, per word class
-            std::vector<int> lnode[9];
             for (int id : leaves) {
                 const Node& nd = nodes[id];
-                if (lane_ok(nd.m)) {
-                    const int nw = ceil_div(nd.m, 32);
-                    LJob j;
-                    memset(&j, 0, sizeof(j));
-                    j.qOff = nd.qOff;
-                    j.tOff = nd.tOff;
-                    j.m = nd.m;
-                    j.n = nd.n;
-                    lj[nw].push_back(j);
-                    lnode[nw].push_back(id);
-                    continue;
-                }
                 WTask t;
                 t.pair = id;
                 t.qOff = nd.qOff;
@@ -827,16 +778,6 @@ void Pass::paths() {
                 tasks.push_back(std::move(t));
             }
             trace.mark("paths: tree + leaf jobs built");
-            for (int nw = 1; nw <= 8; ++nw) {
-                if (lj[nw].empty()) continue;
-                lane_paths(lj[nw], nw, [&](size_t j, const uint8_t* ops, int len, int score) {
-                    Node& nd = nodes[lnode[nw][j]];
-                    if (score != nd.best) throw std::runtime_error("internal: path sweep disagrees with the distance");
-                    nd.opsOff = (long long)opsPool.size();
-                    nd.opsLen = len;
-                    opsPool.insert(opsPool.end(), ops, ops + len);
-                });
-            }
             runner.run(tasks);
             for (const WTask& t : tasks) {
                 Node& nd = nodes[t.pair];

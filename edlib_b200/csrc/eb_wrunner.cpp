@@ -63,6 +63,15 @@ WPlan plan_w_band(int m, long long height, int dhi) {
     return pl;
 }
 
+bool WRunner::lane_ok(int nw) {
+    if (laneOk[nw] < 0) {
+        int bt = 0, rc = 0;
+        be->k1_shape(nw, p->ncodes, 0x7fffffff, &bt, &rc);
+        laneOk[nw] = rc > 0 ? 1 : 0;
+    }
+    return laneOk[nw] == 1;
+}
+
 size_t WRunner::task_bytes(const WTask& t) const {
     size_t b = (size_t)p->ncodes * t.nWp * 4 + sizeof(WJob) + sizeof(Rec);
     if (t.flags & WF_STORE) b += (size_t)t.n * t.nWp * 8 + (size_t)t.m + t.n + 64;
@@ -153,9 +162,7 @@ void WRunner::run(std::vector<WTask>& tasks) {
     }
     for (auto& kv : bands) run_band(tasks, kv.second, kv.first);
     for (auto& kv : lanes) {
-        int bt = 0, rc = 0;
-        be->k1_shape(kv.first.first, p->ncodes, 0x7fffffff, &bt, &rc);
-        if (rc <= 0 || (int)kv.second.size() < 8) {  // alphabet too large for per-thread Peq rows / too few to bother
+        if (!lane_ok(kv.first.first) || (int)kv.second.size() < 8) {  // alphabet too large for per-thread Peq rows / too few to bother
             warp.insert(warp.end(), kv.second.begin(), kv.second.end());
             continue;
         }
@@ -197,6 +204,7 @@ void WRunner::run_lane(std::vector<WTask>& tasks, const std::vector<int>& idx, i
         const int J = (int)(j - i);
         std::vector<LJob> jobs(J);
         std::vector<TbJob> tb;
+        std::vector<int> tbTask;
         uint64_t matEntries = 0, opsBytes = 0;
         for (int s = 0; s < J; ++s) {
             const WTask& t = tasks[idx[i + s]];
@@ -221,6 +229,7 @@ void WRunner::run_lane(std::vector<WTask>& tasks, const std::vector<int>& idx, i
                 b.n = t.n;
                 b.nWp = nw;
                 tb.push_back(b);
+                tbTask.push_back(idx[i + s]);
                 matEntries += (uint64_t)t.n * nw;
                 opsBytes += (uint64_t)t.m + t.n;
             }
@@ -232,41 +241,15 @@ void WRunner::run_lane(std::vector<WTask>& tasks, const std::vector<int>& idx, i
         DevBuf<U2> dMat(be, matEntries);
         LParams lp{dJobs.p, J, p->dSeq.p, p->dSeq.p, p->ncodes, p->hasEq ? p->dEqtab.p : nullptr, dRecs.p, dMat.p, 1};
         be->launch_lane(lp, nw, mode, rev, store);
-        DevBuf<TbJob> dTb;
-        DevBuf<uint8_t> dOps;
-        DevBuf<int> dOpsStart, dOpsLen;
-        if (store) {
-            dTb.alloc(be, tb.size());
-            dTb.upload(tb.data(), tb.size());
-            dOps.alloc(be, opsBytes);
-            dOpsStart.alloc(be, tb.size());
-            dOpsLen.alloc(be, tb.size());
-            TbParams tp{dTb.p, (int)tb.size(), dMat.p, nullptr, p->dSeq.p, p->dSeq.p, p->hasEq ? p->dEqtab.p : nullptr, p->ncodes,
-                        dOps.p, dOpsStart.p, dOpsLen.p, 1};
-            be->launch_traceback(tp);
-        }
-        std::vector<Rec> recs(J);
-        dRecs.download(recs.data(), J);
+        if (store) traceback(tasks, tb, tbTask, dMat.p, nullptr);
+        HostBuf<Rec> recs(be, (size_t)J);
+        dRecs.download(recs.p, J);
         eng->stats.d2hBytes += (long long)J * (long long)sizeof(Rec);
         for (int s = 0; s < J; ++s) {
             WTask& t = tasks[idx[i + s]];
             t.rec = recs[s];
             t.extra.clear();
             if (t.wantPositions && t.rec.cnt > KPOS) spill.push_back(idx[i + s]);
-        }
-        if (store) {
-            std::vector<int> st(tb.size()), ln(tb.size());
-            dOpsStart.download(st.data(), tb.size());
-            dOpsLen.download(ln.data(), tb.size());
-            std::vector<uint8_t> ops(opsBytes);
-            dOps.download(ops.data(), opsBytes);
-            eng->stats.d2hBytes += (long long)opsBytes + 8LL * (long long)tb.size();
-            for (int s = 0; s < J; ++s) {
-                WTask& t = tasks[idx[i + s]];
-                t.opsOff = (long long)opsPool->size();
-                t.opsLen = ln[s];
-                opsPool->insert(opsPool->end(), ops.begin() + tb[s].outOff + st[s], ops.begin() + tb[s].outOff + st[s] + ln[s]);
-            }
         }
         i = j;
     }
@@ -339,20 +322,7 @@ void WRunner::run_slice(std::vector<WTask>& tasks, const std::vector<int>& slice
     be->launch_peq(pp);
     WParams wp{dJobs.p, J, p->dSeq.p, p->dSeq.p, dPeq.p, dH.p, dMat.p, dCol.p, dRecs.p, dOvf.p, dOvfCount.p, ovfCap};
     be->launch_w(wp, R);
-
-    DevBuf<TbJob> dTb;
-    DevBuf<uint8_t> dOps;
-    DevBuf<int> dOpsStart, dOpsLen;
-    if (!tb.empty()) {
-        dTb.alloc(be, tb.size());
-        dTb.upload(tb.data(), tb.size());
-        dOps.alloc(be, opsBytes);
-        dOpsStart.alloc(be, tb.size());
-        dOpsLen.alloc(be, tb.size());
-        TbParams tp{dTb.p, (int)tb.size(), dMat.p, dPeq.p, p->dSeq.p, p->dSeq.p, p->hasEq ? p->dEqtab.p : nullptr, p->ncodes,
-                    dOps.p, dOpsStart.p, dOpsLen.p, 1};
-        be->launch_traceback(tp);
-    }
+    if (!tb.empty()) traceback(tasks, tb, tbTask, dMat.p, dPeq.p);
 
     std::vector<Rec> recs(J);
     dRecs.download(recs.data(), J);
@@ -369,20 +339,6 @@ void WRunner::run_slice(std::vector<WTask>& tasks, const std::vector<int>& slice
         for (const Ovf& o : ov) {
             WTask& t = tasks[slice[o.rec]];
             if (o.score == t.rec.best) t.extra.push_back(o.pos);
-        }
-    }
-    if (!tb.empty()) {
-        std::vector<int> st(tb.size()), ln(tb.size());
-        dOpsStart.download(st.data(), tb.size());
-        dOpsLen.download(ln.data(), tb.size());
-        std::vector<uint8_t> ops(opsBytes);
-        dOps.download(ops.data(), opsBytes);
-        eng->stats.d2hBytes += (long long)opsBytes + 8LL * (long long)tb.size();
-        for (size_t k = 0; k < tb.size(); ++k) {
-            WTask& t = tasks[tbTask[k]];
-            t.opsOff = (long long)opsPool->size();
-            t.opsLen = ln[k];
-            opsPool->insert(opsPool->end(), ops.begin() + tb[k].outOff + st[k], ops.begin() + tb[k].outOff + st[k] + ln[k]);
         }
     }
     if (colInts) {
@@ -427,6 +383,35 @@ void WRunner::run_slice(std::vector<WTask>& tasks, const std::vector<int>& slice
         }
         if (need > 0x7fffffffLL / 4) throw std::runtime_error("end-location list too large");
         if (!again.empty()) run_slice(tasks, again, R, (int)need + 16);
+    }
+}
+
+void WRunner::traceback(std::vector<WTask>& tasks, const std::vector<TbJob>& tb, const std::vector<int>& owner, const U2* mat,
+                        const uint32_t* peq) {
+    const size_t n = tb.size();
+    const uint64_t opsBytes = tb.back().outOff + (uint64_t)tb.back().m + tb.back().n;
+    DevBuf<TbJob> dTb(be, n);
+    dTb.upload(tb.data(), n);
+    DevBuf<uint8_t> dOps(be, opsBytes);
+    DevBuf<int> dStart(be, n), dLen(be, n);
+    TbParams tp{dTb.p, (int)n, mat, peq, p->dSeq.p, p->dSeq.p, p->hasEq ? p->dEqtab.p : nullptr, p->ncodes,
+                dOps.p, dStart.p, dLen.p, 1};
+    be->launch_traceback(tp);
+    // one pinned staging block for everything that comes back (fast D2H, no zero-fill of vectors)
+    const size_t offLn = round_up(n * sizeof(int), 64), offOps = offLn + round_up(n * sizeof(int), 64);
+    HostBuf<uint8_t> host(be, offOps + opsBytes);
+    const int* st = reinterpret_cast<const int*>(host.p);
+    const int* ln = reinterpret_cast<const int*>(host.p + offLn);
+    const uint8_t* ops = host.p + offOps;
+    be->d2h(host.p, dStart.p, n * sizeof(int));
+    be->d2h(host.p + offLn, dLen.p, n * sizeof(int));
+    be->d2h(host.p + offOps, dOps.p, opsBytes);
+    eng->stats.d2hBytes += (long long)opsBytes + 8LL * (long long)n;
+    for (size_t q = 0; q < n; ++q) {
+        WTask& t = tasks[owner[q]];
+        t.opsOff = (long long)opsPool->size();
+        t.opsLen = ln[q];
+        opsPool->insert(opsPool->end(), ops + tb[q].outOff + st[q], ops + tb[q].outOff + st[q] + ln[q]);
     }
 }
 }  // namespace eb

@@ -110,6 +110,33 @@ def path_cases(seed, count):
         yield dict(q=q, t=t, k=-1, mode=rng.choice([0, 0, 1, 2]), task=2, eqs=None)
 
 
+def path_batch_cases(seed, count):
+    """path_cases in batches of 24-40 pairs of one mode: the short-row Hirschberg leaves of many trees are swept
+    together, some word classes with enough of them for the lane kernel."""
+    rng = random.Random(seed)
+    for b in range(count):
+        pairs = list(path_cases(seed * 1000 + b, rng.randrange(24, 41)))
+        yield dict(qs=[c["q"] for c in pairs], ts=[c["t"] for c in pairs], k=-1, mode=rng.choice([0, 0, 1, 2]), task=2, eqs=None)
+
+
+def long_target_path_cases(seed, count):
+    """NW PATH batches of short queries (<= 256 rows), each against its own target of 3-8 times 32 symbols per query word:
+    an NW path spans the whole target, longer than a device-driven path slice may be, so every pair takes the host tree
+    (one leaf each).  Two word classes of a batch hold 8 or more pairs, two hold fewer."""
+    rng = random.Random(seed)
+    for _ in range(count):
+        alpha = bytes(rng.sample(range(256), rng.choice([2, 4, 4, 20])))
+        qs, ts = [], []
+        for nw, num in zip(rng.sample(range(1, 9), 4), (rng.randrange(8, 16), rng.randrange(8, 16), rng.randrange(1, 8), rng.randrange(1, 8))):
+            for _ in range(num):
+                t = rand_seq(rng, 32 * nw * rng.randrange(3, 9) + rng.randrange(32), alpha)
+                m = rng.randrange(32 * nw - 31, 32 * nw + 1)
+                a = rng.randrange(0, len(t) - m)
+                qs.append(mutate(rng, t[a:a + m + 8], rng.choice([0, 0.05, 0.3]), alpha)[:m])
+                ts.append(t)
+        yield dict(qs=qs, ts=ts, k=-1, mode=0, task=2, eqs=None)
+
+
 def filter_cases(seed, count):
     """HW batches of reads (>= 48 bp) over one shared target: clean hits, hits above the filter
     thresholds, unrelated reads, exact copies inside repeated target segments (several far-apart or
