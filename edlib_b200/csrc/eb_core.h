@@ -1064,7 +1064,7 @@ EB_HD void win_reduce_read(const WinReduceParams& p, int slot) {
             }
         }
     }
-    if (p.leftover) {  // device-driven first level: the outcome logic of Pass::seed_stage, per read
+    if (p.leftover) {  // device-driven first level: the outcome logic of Pass::window_outcomes, per read
         const int pair = p.readList ? p.readList[slot] : p.firstPair + slot;
         const int m = p.qlen[pair];
         const int bound = (p.kBound < 0 || p.kBound > m) ? m : p.kBound;

@@ -624,9 +624,15 @@ struct Pass {
     void lane_merge(LaneGroup& c, const std::vector<int>& sub, int chunks, const std::vector<Rec>& rr, const std::vector<Ovf>* oo,
                     std::vector<int>& incomplete, long long& missing);
 
-    // It is now known that read s has no alignment within t: final if t is the caller's bound, else the
-    // read moves on to `next`.
-    void no_distance_within(LaneGroup& c, int s, int t, std::vector<int>& next);
+    // The outcome of `pair` is "no alignment within its bound": no distance, no end columns.
+    void no_alignment(int pair) {
+        best[pair] = 0x7fffffff;
+        cnt[pair] = 0;
+        posLen[pair] = 0;
+    }
+    // It is now known that read s has no alignment within t.  Returns whether that is final (t is the read's bound: its
+    // outcome is set); otherwise the read goes on to a later stage.
+    bool no_distance_within(LaneGroup& c, int s, int t);
 
     // Strand batches: the cross-strand rule (eb_core.h: strand_rule) over the reads of `list` whose other strand is in
     // the list as well (at s + 1 for a forward pair s).  The reads of the `pending` lists are undecided (excl / bound
@@ -638,16 +644,20 @@ struct Pass {
     // becomes "no alignment", so that start locations and paths are only computed for winners.
     void pick_strands();
 
+    // Outcome of the reads `cand` (indices into `list`) of a window stage, with thresholds thr[i] (< 0: the stage left
+    // the read out, it goes on), their plans on the device and the records of their swept windows: the reduction
+    // (win_reduce), then per read decided (best / cnt / end columns), no distance within thr[i] (no_distance_within),
+    // on to `next` (saturated) or to c.direct (long end-location list).  Counts the last two in nSat / nLong.
+    void window_outcomes(LaneGroup& c, const std::vector<int>& cand, const int* thr, const SeedPlan* plan, const WinRecords& wr,
+                         std::vector<int>& next, int& nSat, int& nLong);
+
     // Seed stage, host-driven: exact seeds of every read looked up in the index of the target; windows around
-    // the expected end columns are planned, swept and reduced on the device (eb_core.h: seed_plan_read), the
-    // outcome per read is worked out on the host.
+    // the expected end columns are planned, swept and reduced on the device (eb_core.h: seed_plan_read).
     void seed_stage(LaneGroup& c, int level, const std::vector<int>& in, std::vector<int>& next);
 
     // Prefix stage over the reads `in` (indices into `list`): a sweep of the first P rows of every read reports
     // the target ranges where that prefix matches within t = min(K0, bound); the whole read is then swept over
-    // one window per range.  A read is decided when a window holds a distance <= t (or when t is the caller's
-    // bound and none does).  Undecided reads go to `next` (a longer prefix or the plain sweep), reads with
-    // long end-location lists to c.direct.
+    // one window per range, and the windows are reduced as those of a seed stage (window_outcomes).
     void prefix_stage(LaneGroup& c, int P, int K0, const std::vector<int>& in, std::vector<int>& next);
 
     // The plain lane-per-alignment sweep of the reads in c.direct over the whole target.

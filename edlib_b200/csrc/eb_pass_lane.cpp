@@ -310,17 +310,12 @@ void Pass::lane_merge(LaneGroup& c, const std::vector<int>& sub, int chunks, con
     }
 }
 
-// It is now known that read s has no alignment within t: final if t is the caller's bound, else the
-// read moves on to `next`.
-void Pass::no_distance_within(LaneGroup& c, int s, int t, std::vector<int>& next) {
+// It is now known that read s has no alignment within t: final if t is the read's bound, else the read goes on.
+bool Pass::no_distance_within(LaneGroup& c, int s, int t) {
     if (t > c.excl[s]) c.excl[s] = t;
-    if (t == c.bound[s]) {
-        best[c.list[s]] = 0x7fffffff;
-        cnt[c.list[s]] = 0;
-        stats.filterDecided++;
-    } else {
-        next.push_back(s);
-    }
+    if (t != c.bound[s]) return false;
+    no_alignment(c.list[s]);
+    return true;
 }
 
 void Pass::strand_prune(const std::vector<int>& list, const std::vector<int>& excl, std::vector<int>& bound,
@@ -344,10 +339,7 @@ void Pass::strand_prune(const std::vector<int>& list, const std::vector<int>& ex
         bound[s] = bd[0];
         bound[s + 1] = bd[1];
         if (loser < 0) continue;
-        const int pair = list[s + loser];
-        best[pair] = 0x7fffffff;
-        cnt[pair] = 0;
-        posLen[pair] = 0;
+        no_alignment(list[s + loser]);
         state[s + loser] = 2;
         stats.filterDecided++;
         lost = true;
@@ -356,69 +348,21 @@ void Pass::strand_prune(const std::vector<int>& list, const std::vector<int>& ex
     for (std::vector<int>* v : pending) v->erase(std::remove_if(v->begin(), v->end(), [&](int s) { return state[s] == 2; }), v->end());
 }
 
-// Seed stage, host-driven: exact seeds of every read looked up in the index of the target; windows around
-// the expected end columns are planned, swept and reduced on the device (eb_core.h: seed_plan_read).
-void Pass::seed_stage(LaneGroup& c, int level, const std::vector<int>& in, std::vector<int>& next) {
+// Outcome of the reads of a window stage (seed or prefix stage): their windows reduced on the device (eb_core.h:
+// win_reduce_read), then the switch on each read's reduced record.
+void Pass::window_outcomes(LaneGroup& c, const std::vector<int>& cand, const int* thr, const SeedPlan* plan, const WinRecords& wr,
+                           std::vector<int>& next, int& nSat, int& nLong) {
     const std::vector<int>& list = c.list;
-    const Target& tg = c.tg;
-    const int nw = c.nw;
-    const std::vector<int>& bound = c.bound;
-    std::vector<int>& excl = c.excl;
-    std::vector<int>& direct = c.direct;
-    if (!seed_index(c.t) || seedIdx->Ls[level] <= 0) {
-        next = in;
-        return;
-    }
-    const int L = seedIdx->Ls[level];
-    // every read of `in` gets a slot; thr < 0 marks the ones this stage cannot help (the kernel skips them)
-    const std::vector<int>& cand = in;
     const int g = (int)cand.size();
-    if (g == 0) return;
-    HostBuf<int> rl(be, g), hThr(be, g);
-    const int* thr = hThr.p;
-    parallel_ranges((size_t)g, 65536, [&](size_t lo, size_t hi) {
-        for (size_t i = lo; i < hi; ++i) {
-            const int s = cand[i];
-            rl[i] = list[s];
-            hThr[i] = seed_threshold(p->qlen[list[s]], bound[s], L, tun.filterSeedK, excl[s]);
-        }
-    });
-    DevBuf<int> dList(be, g), dThr(be, g), dCount(be, 1);
-    dList.upload(rl.p, g);
-    dThr.upload(hThr.p, g);
-    DevBuf<SeedPlan> dPlan(be, g);
-    // room for the window jobs: sized from what the previous pass of this level needed per read
-    int& perRead = eng.scratch.seedWindowsPerRead[level];
-    const int cap = (int)std::min<long long>((long long)g * std::max(perRead + 2, level == 0 ? 8 : level == 1 ? 96 : level == 2 ? 400 : 1500) + 4096, 1LL << 28);
-    SeedPlanParams sp = seed_plan_params(tg, level);
-    sp.readList = dList.p;
-    sp.thr = dThr.p;
-    sp.numReads = g;
-    sp.maxLen = 32 * nw;
-    sp.plan = dPlan.p;
-    WinJobs jobs;
-    jobs.count = dCount.p;
-    be->zero(dCount.p, sizeof(int));
-    const int V = plan_windows(sp, jobs, cap, true);
-    perRead = (int)(((long long)V + g - 1) / g);
-    stats.filterWindows += V;
-    trace.mark("filter: seeds planned");
-    DevBuf<WinRec> dWinRecs(be, (size_t)std::max(V, 1));
-    // end columns beyond the inline ones of a window (reads that tie on many end columns)
-    const int ovfCap = (int)std::min<long long>((long long)V / 8 + 65536, 1 << 24);
-    DevBuf<Ovf> dOvf(be, (size_t)ovfCap);
-    DevBuf<int> dOvfCount(be, 1);
-    be->zero(dOvfCount.p, sizeof(int));
-    const WinRecords wr{dWinRecs.p, dOvf.p, dOvfCount.p, ovfCap};
-    if (V > 0) sweep_windows(tg, nw, jobs, V, wr);
     DevBuf<Rec> dOut(be, g);
+    DevBuf<int> dCount(be, 1);
     int extraCap = g / 4 + 16384;
     DevBuf<int> dExtra;
     int nExtra = 0;
     for (;;) {
         dExtra.alloc(be, (size_t)extraCap);
         be->zero(dCount.p, sizeof(int));
-        reduce_windows(WinReduceParams{}, dPlan.p, g, wr, dOut.p, dExtra.p, dCount.p, extraCap);
+        reduce_windows(WinReduceParams{}, plan, g, wr, dOut.p, dExtra.p, dCount.p, extraCap);
         dCount.download(&nExtra, 1);
         if (nExtra <= extraCap) break;
         extraCap = nExtra;  // the extra list ran over (repeat-rich reads): reduce again with the exact size
@@ -428,9 +372,10 @@ void Pass::seed_stage(LaneGroup& c, int level, const std::vector<int>& in, std::
     std::vector<int> extra((size_t)nExtra);
     if (nExtra) dExtra.download(extra.data(), (size_t)nExtra);
     stats.d2hBytes += (long long)g * (long long)sizeof(Rec) + 4 + 4LL * nExtra;
-    trace.mark("filter: seed windows");
+    trace.mark("filter: windows reduced");
     // Outcome per read, on a few host threads: records of decided reads go straight to best / cnt;
     // their positions are appended to posPool in slot order (counts first, then the fill).
+    // c.repeat is read between the seed levels and the prefix stages only: what the prefix stages write to it is unused.
     struct Part {
         std::vector<int> next, direct;
         long long decided = 0, positions = 0;
@@ -459,14 +404,8 @@ void Pass::seed_stage(LaneGroup& c, int level, const std::vector<int>& in, std::
                 P.positions += r.cnt;
             } else if (r.rsv == SEED_NONE) {
                 c.repeat[s] = 0;
-                if (thr[i] > excl[s]) excl[s] = thr[i];
-                if (thr[i] == bound[s]) {  // nothing within the caller's bound: final
-                    best[pair] = 0x7fffffff;
-                    cnt[pair] = 0;
-                    P.decided++;
-                } else {
-                    P.next.push_back(s);
-                }
+                if (no_distance_within(c, s, thr[i])) P.decided++;
+                else P.next.push_back(s);
             } else if (r.rsv == SEED_LONG_LIST) {
                 P.direct.push_back(s);
                 P.nLong++;
@@ -477,7 +416,6 @@ void Pass::seed_stage(LaneGroup& c, int level, const std::vector<int>& in, std::
             }
         }
     });
-    int nSat = 0, nLong = 0;
     std::vector<long long> partPos(parts.size());
     {
         long long at = (long long)posPool.size();
@@ -488,7 +426,7 @@ void Pass::seed_stage(LaneGroup& c, int level, const std::vector<int>& in, std::
             nSat += parts[t2].nSat;
             nLong += parts[t2].nLong;
             next.insert(next.end(), parts[t2].next.begin(), parts[t2].next.end());
-            direct.insert(direct.end(), parts[t2].direct.begin(), parts[t2].direct.end());
+            c.direct.insert(c.direct.end(), parts[t2].direct.begin(), parts[t2].direct.end());
         }
         posPool.resize((size_t)at);
     }
@@ -503,6 +441,60 @@ void Pass::seed_stage(LaneGroup& c, int level, const std::vector<int>& in, std::
             for (int q = KPOS; q < r.cnt; ++q) posPool[(size_t)at++] = extra[(size_t)r.last + q - KPOS];
         }
     });
+}
+
+// Seed stage, host-driven: exact seeds of every read looked up in the index of the target; windows around
+// the expected end columns are planned, swept and reduced on the device (eb_core.h: seed_plan_read).
+void Pass::seed_stage(LaneGroup& c, int level, const std::vector<int>& in, std::vector<int>& next) {
+    const std::vector<int>& list = c.list;
+    const Target& tg = c.tg;
+    const int nw = c.nw;
+    if (!seed_index(c.t) || seedIdx->Ls[level] <= 0) {
+        next = in;
+        return;
+    }
+    const int L = seedIdx->Ls[level];
+    // every read of `in` gets a slot; thr < 0 marks the ones this stage cannot help (the kernel skips them)
+    const int g = (int)in.size();
+    if (g == 0) return;
+    HostBuf<int> rl(be, g), thr(be, g);
+    parallel_ranges((size_t)g, 65536, [&](size_t lo, size_t hi) {
+        for (size_t i = lo; i < hi; ++i) {
+            const int s = in[i];
+            rl[i] = list[s];
+            thr[i] = seed_threshold(p->qlen[list[s]], c.bound[s], L, tun.filterSeedK, c.excl[s]);
+        }
+    });
+    DevBuf<int> dList(be, g), dThr(be, g), dCount(be, 1);
+    dList.upload(rl.p, g);
+    dThr.upload(thr.p, g);
+    DevBuf<SeedPlan> dPlan(be, g);
+    // room for the window jobs: sized from what the previous pass of this level needed per read
+    int& perRead = eng.scratch.seedWindowsPerRead[level];
+    const int cap = (int)std::min<long long>((long long)g * std::max(perRead + 2, level == 0 ? 8 : level == 1 ? 96 : level == 2 ? 400 : 1500) + 4096, 1LL << 28);
+    SeedPlanParams sp = seed_plan_params(tg, level);
+    sp.readList = dList.p;
+    sp.thr = dThr.p;
+    sp.numReads = g;
+    sp.maxLen = 32 * nw;
+    sp.plan = dPlan.p;
+    WinJobs jobs;
+    jobs.count = dCount.p;
+    be->zero(dCount.p, sizeof(int));
+    const int V = plan_windows(sp, jobs, cap, true);
+    perRead = (int)(((long long)V + g - 1) / g);
+    stats.filterWindows += V;
+    trace.mark("filter: seeds planned");
+    DevBuf<WinRec> dWinRecs(be, (size_t)std::max(V, 1));
+    // end columns beyond the inline ones of a window (reads that tie on many end columns)
+    const int ovfCap = (int)std::min<long long>((long long)V / 8 + 65536, 1 << 24);
+    DevBuf<Ovf> dOvf(be, (size_t)ovfCap);
+    DevBuf<int> dOvfCount(be, 1);
+    be->zero(dOvfCount.p, sizeof(int));
+    const WinRecords wr{dWinRecs.p, dOvf.p, dOvfCount.p, ovfCap};
+    if (V > 0) sweep_windows(tg, nw, jobs, V, wr);
+    int nSat = 0, nLong = 0;
+    window_outcomes(c, in, thr.p, dPlan.p, wr, next, nSat, nLong);
     if (trace.on) {
         int nOvf = 0;
         dOvfCount.download(&nOvf, 1);
@@ -522,8 +514,7 @@ void Pass::prefix_stage(LaneGroup& c, int P, int K0, const std::vector<int>& in,
     const int n = c.n;
     const int nw = c.nw;
     const std::vector<int>& bound = c.bound;
-    std::vector<int>& excl = c.excl;
-    std::vector<int>& direct = c.direct;
+    const std::vector<int>& excl = c.excl;
     std::vector<int> cand, thr;
     const int minLen = std::max(tun.filterMinLen * P / 64, P + 1);
     for (int s : in) {
@@ -543,7 +534,6 @@ void Pass::prefix_stage(LaneGroup& c, int P, int K0, const std::vector<int>& in,
     std::vector<Ovf> ranges;
     lane_sweep(c, cand, thr, P / 32, chunksA, chunkLenA, (int)std::min<long long>(16LL * g + 4096, 1LL << 28), P, 1, none, ranges);
     trace.mark("filter: prefix sweep");
-    auto undecided = [&](int s, int t) { no_distance_within(c, s, t, next); };
     // ranges of every read, ascending (the list is in completion order)
     std::vector<int> start(g + 1, 0);
     std::vector<char> saturated(g, 0);
@@ -558,18 +548,17 @@ void Pass::prefix_stage(LaneGroup& c, int P, int K0, const std::vector<int>& in,
         for (const Ovf& o : ranges)
             if (o.score >= 0) rg[fill[o.rec]++] = std::make_pair(o.score, o.pos);
     }
-    std::vector<int> vOwner, vPair, vK, vWs, vLen, vTf;  // windows to verify
-    std::vector<int> wFirst(g + 1, 0);
+    // windows to verify, and the plan of every read: its windows, none (no range or no window: nothing within t),
+    // or saturated (its range list ran over, or too many windows: on to the next stage)
+    std::vector<int> vPair, vK, vWs, vLen, vTf;
+    std::vector<SeedPlan> plan(g);
     for (int i = 0; i < g; ++i) {
-        wFirst[i] = (int)vOwner.size();
         const int s = cand[i];
         const int pair = list[s], m = p->qlen[pair], t = thr[i];
+        const int w0 = (int)vPair.size();
+        plan[i] = SeedPlan{w0, 0, SEED_NONE, t};
         if (saturated[i]) {
-            next.push_back(s);
-            continue;
-        }
-        if (start[i] == start[i + 1]) {
-            undecided(s, t);
+            plan[i].state = SEED_SATURATED;
             continue;
         }
         std::sort(rg.begin() + start[i], rg.begin() + start[i + 1]);
@@ -578,7 +567,6 @@ void Pass::prefix_stage(LaneGroup& c, int P, int K0, const std::vector<int>& in,
         // columns to examine are [first+(m-P)-t, last+(m-P)+t] of every range.  Ranges close to
         // each other share one window; tracked columns of successive windows are kept disjoint.
         long long prevHi = -1;
-        int windows = 0;
         for (int a = start[i]; a < start[i + 1];) {
             const int first = rg[a].first;
             int last = rg[a].second;
@@ -597,101 +585,54 @@ void Pass::prefix_stage(LaneGroup& c, int P, int K0, const std::vector<int>& in,
             prevHi = hi;
             // HW restart: alignments with <= t edits span at most m + t columns (scores <= t stay exact)
             const long long ws = std::max<long long>(0, lo - (long long)(m + t)) & ~15LL;  // windows start at multiples of 16
-            vOwner.push_back(i);
             vPair.push_back(pair);
             vK.push_back(t + 1);
             vWs.push_back((int)ws);
             vLen.push_back((int)(hi - ws + 1));
             vTf.push_back((int)(lo - ws));
-            ++windows;
         }
-        if (windows == 0) {
-            undecided(s, t);
-        } else if (windows > tun.filterMaxWindows) {
-            vOwner.resize(wFirst[i]);
-            vPair.resize(wFirst[i]);
-            vK.resize(wFirst[i]);
-            vWs.resize(wFirst[i]);
-            vLen.resize(wFirst[i]);
-            vTf.resize(wFirst[i]);
-            next.push_back(s);
+        const int windows = (int)vPair.size() - w0;
+        if (windows > tun.filterMaxWindows) {
+            vPair.resize(w0);
+            vK.resize(w0);
+            vWs.resize(w0);
+            vLen.resize(w0);
+            vTf.resize(w0);
+            plan[i].state = SEED_SATURATED;
+        } else if (windows > 0) {
+            plan[i].count = windows;
+            plan[i].state = SEED_WINDOWS;
         }
     }
-    wFirst[g] = (int)vOwner.size();
     trace.mark("filter: windows planned");
-    const int V = (int)vOwner.size();
+    const int V = (int)vPair.size();
     stats.filterWindows += V;
-    if (trace.on) {
-        int sat = 0;
-        for (char c : saturated) sat += c;
-        fprintf(stderr, "[edlib_b200] filter stage P=%d: %d reads, %zu ranges, %d saturated, %d windows, %zu to the next stage\n",
-                P, g, rg.size(), sat, V, next.size());
-    }
-    if (V == 0) return;
-    // Whole reads over their windows, one window per thread (k1w_kernel).
-    WinJobs jobs;
-    jobs.alloc(be, V);
-    jobs.pair.upload(vPair.data(), V);
-    jobs.k.upload(vK.data(), V);
-    jobs.start.upload(vWs.data(), V);
-    jobs.len.upload(vLen.data(), V);
-    jobs.tf.upload(vTf.data(), V);
+    // Whole reads over their windows, one window per thread (k1w_kernel), reduced per read as in a seed stage.
+    DevBuf<SeedPlan> dPlan(be, g);
+    dPlan.upload(plan.data(), g);
     DevBuf<WinRec> dRecs(be, V);
     const int ovfCap = (int)std::min<long long>((long long)V / 8 + 65536, 1 << 24);
     DevBuf<Ovf> dOvf(be, (size_t)ovfCap);
     DevBuf<int> dOvfCount(be, 1);
     be->zero(dOvfCount.p, sizeof(int));
-    sweep_windows(tg, nw, jobs, V, WinRecords{dRecs.p, dOvf.p, dOvfCount.p, ovfCap});
-    std::vector<WinRec> rv(V);
-    dRecs.download(rv.data(), V);
-    int nOvf = 0;
-    dOvfCount.download(&nOvf, 1);
-    const bool ovfComplete = nOvf <= ovfCap;
-    std::vector<Ovf> ovf((size_t)std::min(nOvf, ovfCap));
-    if (!ovf.empty()) dOvf.download(ovf.data(), ovf.size());
-    stats.d2hBytes += (long long)V * (long long)sizeof(WinRec) + 4 + (long long)ovf.size() * (long long)sizeof(Ovf);
-    trace.mark("filter: window sweeps");
-    // end columns beyond the inline ones, per window, in sweep order (entries of another score are stale)
-    std::unordered_map<int, std::vector<int>> listed;
-    for (const Ovf& o : ovf)
-        if (o.rec >= 0 && o.rec < V && o.score == rv[o.rec].best) listed[o.rec].push_back(o.pos);
-    for (int i = 0; i < g; ++i) {
-        if (wFirst[i] == wFirst[i + 1]) continue;
-        const int s = cand[i], t = thr[i], pair = list[s];
-        int b = 0x7fffffff;
-        for (int j = wFirst[i]; j < wFirst[i + 1]; ++j)
-            if (rv[j].cnt > 0 && rv[j].best < b) b = rv[j].best;
-        if (b > t) {  // every window minimum is above the threshold
-            undecided(s, t);
-            continue;
-        }
-        bool longList = false;
-        int total = 0;
-        for (int j = wFirst[i]; j < wFirst[i + 1]; ++j)
-            if (rv[j].cnt > 0 && rv[j].best == b) {
-                total += rv[j].cnt;
-                if (rv[j].cnt > KPOSW) {
-                    auto it = listed.find(j);
-                    if (!ovfComplete || it == listed.end() || (int)it->second.size() != rv[j].cnt - KPOSW) longList = true;
-                }
-            }
-        if (longList) {  // the list ran over: the plain sweep collects the columns
-            direct.push_back(s);
-            continue;
-        }
-        stats.filterDecided++;
-        best[pair] = b;
-        cnt[pair] = total;
-        posStart[pair] = (long long)posPool.size();
-        for (int j = wFirst[i]; j < wFirst[i + 1]; ++j)
-            if (rv[j].cnt > 0 && rv[j].best == b) {
-                for (int q = 0; q < std::min(rv[j].cnt, KPOSW); ++q) posPool.push_back(rv[j].pos[q]);
-                if (rv[j].cnt > KPOSW) {
-                    const std::vector<int>& ex = listed[j];
-                    posPool.insert(posPool.end(), ex.begin(), ex.end());
-                }
-            }
-        posLen[pair] = total;
+    const WinRecords wr{dRecs.p, dOvf.p, dOvfCount.p, ovfCap};
+    WinJobs jobs;
+    if (V > 0) {
+        jobs.alloc(be, V);
+        jobs.pair.upload(vPair.data(), V);
+        jobs.k.upload(vK.data(), V);
+        jobs.start.upload(vWs.data(), V);
+        jobs.len.upload(vLen.data(), V);
+        jobs.tf.upload(vTf.data(), V);
+        sweep_windows(tg, nw, jobs, V, wr);
+    }
+    int nSat = 0, nLong = 0;
+    window_outcomes(c, cand, thr.data(), dPlan.p, wr, next, nSat, nLong);
+    if (trace.on) {
+        int sat = 0;
+        for (char x : saturated) sat += x;
+        fprintf(stderr, "[edlib_b200] filter stage P=%d: %d reads, %zu ranges, %d saturated, %d windows, %zu to the next stage\n",
+                P, g, rg.size(), sat, V, next.size());
     }
 }
 

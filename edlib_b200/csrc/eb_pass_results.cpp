@@ -29,13 +29,24 @@ void Pass::long_hw_distance(const std::vector<int>& pairs) {
             cur[s] = s;
             stats.wCells += (long long)m * n;
         }
-        auto decide = [&](int s, int b, int c, const std::vector<int>& positions) {
+        // The minimum over the tasks [q0, q1) of query s, when it is below `limit`, becomes the query's outcome, with the end
+        // columns of the tasks attaining it (task columns shifted by the task's tag to target columns).
+        auto take_minimum = [&](const std::vector<WTask>& tasks, int q0, int q1, int s, int limit) {
+            int b = 0x7fffffff;
+            for (int q = q0; q < q1; ++q)
+                if (tasks[q].rec.cnt > 0 && tasks[q].rec.best < b) b = tasks[q].rec.best;
+            if (b >= limit) return false;
             const int pair = list[s];
-            best[pair] = c > 0 ? b : 0x7fffffff;
-            cnt[pair] = c;
             posStart[pair] = (long long)posPool.size();
-            posPool.insert(posPool.end(), positions.begin(), positions.end());
-            posLen[pair] = (int)positions.size();
+            for (int q = q0; q < q1; ++q) {
+                const WTask& tk = tasks[q];
+                if (tk.rec.cnt <= 0 || tk.rec.best != b) continue;
+                for (int x = 0; x < std::min(tk.rec.cnt, KPOS); ++x) posPool.push_back(tk.tag + tk.rec.pos[x]);
+                for (int x : tk.extra) posPool.push_back(tk.tag + x);
+            }
+            best[pair] = b;
+            cnt[pair] = posLen[pair] = (int)((long long)posPool.size() - posStart[pair]);
+            return true;
         };
         // ---- seed levels with doubling thresholds ----
         const bool seeds = !p->hasEq && tun.filterSeedK > 0 && tun.longSeedMaxK > 0 && n >= tun.filterMinTarget && seed_index(t) &&
@@ -128,24 +139,13 @@ void Pass::long_hw_distance(const std::vector<int>& pairs) {
                     rest.push_back(s);
                     continue;
                 }
-                int b = 0x7fffffff;
-                for (int q = taskFirst[i]; q < taskFirst[i + 1]; ++q)
-                    if (tasks[q].rec.cnt > 0 && tasks[q].rec.best < b) b = tasks[q].rec.best;
-                if (b <= tt) {
-                    std::vector<int> positions;
-                    for (int q = taskFirst[i]; q < taskFirst[i + 1]; ++q) {
-                        const WTask& tk = tasks[q];
-                        if (tk.rec.cnt <= 0 || tk.rec.best != b) continue;
-                        for (int x = 0; x < std::min(tk.rec.cnt, KPOS); ++x) positions.push_back(tk.tag + tk.rec.pos[x]);
-                        for (int x : tk.extra) positions.push_back(tk.tag + x);
-                    }
-                    decide(s, b, (int)positions.size(), positions);
+                if (take_minimum(tasks, taskFirst[i], taskFirst[i + 1], s, tt + 1)) {
                     stats.filterDecided++;
                     continue;
                 }
                 excl[s] = tt;  // no alignment within tt
                 if (tt == bound[s]) {
-                    decide(s, 0, 0, std::vector<int>());  // ... which is the caller's bound: final
+                    no_alignment(list[s]);  // ... which is the caller's bound: final
                     stats.filterDecided++;
                 } else if (top[i] > tt) {
                     cur.push_back(s);  // next level: twice the threshold
@@ -196,19 +196,8 @@ void Pass::long_hw_distance(const std::vector<int>& pairs) {
         taskFirst[cur.size()] = (int)tasks.size();
         runner.run(tasks);
         if (trace.on) fprintf(stderr, "[edlib_b200] long HW queries, chunked sweeps: %zu queries, %zu chunks\n", cur.size(), tasks.size());
-        for (size_t i = 0; i < cur.size(); ++i) {
-            int b = 0x7fffffff;
-            for (int q = taskFirst[i]; q < taskFirst[i + 1]; ++q)
-                if (tasks[q].rec.cnt > 0 && tasks[q].rec.best < b) b = tasks[q].rec.best;
-            std::vector<int> positions;
-            for (int q = taskFirst[i]; q < taskFirst[i + 1]; ++q) {
-                const WTask& tk = tasks[q];
-                if (tk.rec.cnt <= 0 || tk.rec.best != b) continue;
-                for (int x = 0; x < std::min(tk.rec.cnt, KPOS); ++x) positions.push_back(tk.tag + tk.rec.pos[x]);
-                for (int x : tk.extra) positions.push_back(tk.tag + x);
-            }
-            decide(cur[i], b, (int)positions.size(), positions);
-        }
+        for (size_t i = 0; i < cur.size(); ++i)  // any minimum found is the query's
+            if (!take_minimum(tasks, taskFirst[i], taskFirst[i + 1], cur[i], 0x7fffffff)) no_alignment(list[cur[i]]);
     }
 }
 

@@ -104,9 +104,14 @@ def test_candidate_filter_all_branches():
                   {"EDLIB_B200_DEVICE_STAGE": "0"},                                   # every stage host-driven
                   {"EDLIB_B200_TINY_SWEEP_READS": "8", "EDLIB_B200_FILTER_SEED_K": "2"},  # few undecided reads: (read, chunk) lane jobs
                   {"EDLIB_B200_SLICE_READS": "64", "EDLIB_B200_FILTER_SEED_LEVELS": "1"}):  # many slices, one seed level
+        prefix_only = extra.get("EDLIB_B200_FILTER_SEED_K") == "0"
         env = dict(os.environ, EDLIB_B200_FILTER_MIN_TARGET="128", EDLIB_B200_FILTER_MIN_LEVEL_READS="0", EDLIB_B200_K1_MIN_GROUP="4", **extra)
+        if prefix_only:
+            env["EDLIB_B200_TRACE"] = "1"
         out = subprocess.run(["python", "-c", code], env=env, check=True, capture_output=True, text=True)
         assert int(out.stdout.strip().splitlines()[-1]) > 500
+        if prefix_only:
+            assert "filter stage P=" in out.stderr  # the prefix stages ran
 
 
 def test_tightest_bounds_through_every_filter_path():
@@ -139,9 +144,14 @@ def test_reads_that_tie_on_many_end_columns():
     for extra in ({"EDLIB_B200_STREAM_MIN_PAIRS": "8"}, {"EDLIB_B200_DEVICE_STAGE": "0"},
                   {"EDLIB_B200_FILTER_SEED_K": "0", "EDLIB_B200_FILTER_K1": "12"},
                   {"EDLIB_B200_STREAM_MIN_PAIRS": "8", "EDLIB_B200_SLICE_READS": "64", "EDLIB_B200_FILTER_SEED_BUCKET": "4096"}):
+        prefix_only = extra.get("EDLIB_B200_FILTER_SEED_K") == "0"
         env = dict(os.environ, EDLIB_B200_FILTER_MIN_TARGET="128", EDLIB_B200_FILTER_MIN_LEVEL_READS="0", EDLIB_B200_K1_MIN_GROUP="4", **extra)
+        if prefix_only:
+            env["EDLIB_B200_TRACE"] = "1"
         out = subprocess.run(["python", "-c", code], env=env, check=True, capture_output=True, text=True)
         assert int(out.stdout.strip().splitlines()[-1]) > 300
+        if prefix_only:
+            assert "filter stage P=" in out.stderr  # the prefix stages ran
 
 
 def test_start_locations_and_paths_driven_from_the_device():
