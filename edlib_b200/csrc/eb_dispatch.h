@@ -2,6 +2,7 @@
 // (eb_kernels.cu) and the CPU emulation (tests/emul/emul_backend.cpp) both select through these, so they accept the
 // same values and instantiate the same classes.  Plain C++17, no CUDA.
 #pragma once
+#include <algorithm>
 #include <stdexcept>
 #include <type_traits>
 
@@ -58,6 +59,24 @@ void with_seed_cap(int level, F&& f) {
     if (level <= 0) f(std::integral_constant<int, SEED_CAND_0>{});
     else if (level == 1) f(std::integral_constant<int, SEED_CAND_1>{});
     else f(std::integral_constant<int, SEED_CAND_2>{});
+}
+
+// Instance of the seed planning kernel for a launch (eb_kernels.cu: seed_plan_kernel<CAP, THREADS, CoopGroup<GW>>):
+// f(cap, threads, gw), each an integral constant.  A read has t + 1 <= min(maxLen / Ls, seedK + 1) seeds: groups of
+// 16 lanes look them all up in one round when that is at most 16, whole warps otherwise (or when the read lengths
+// are not known); the last level is planned by a warp per read, two reads per CTA.
+template <class F>
+void with_seed_plan_instance(const SeedPlanParams& p, F&& f) {
+    const bool narrow = p.maxLen > 0 && p.Ls > 0 && std::min(p.maxLen / p.Ls, p.seedK + 1) <= 16;
+    with_seed_cap(p.level, [&](auto cap) {
+        using I64 = std::integral_constant<int, 64>;
+        using I128 = std::integral_constant<int, 128>;
+        using I16 = std::integral_constant<int, 16>;
+        using I32 = std::integral_constant<int, 32>;
+        if constexpr (decltype(cap)::value == SEED_CAND_2) f(cap, I64{}, I32{});
+        else if (narrow) f(cap, I128{}, I16{});
+        else f(cap, I128{}, I32{});
+    });
 }
 
 }  // namespace eb

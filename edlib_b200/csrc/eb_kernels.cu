@@ -976,6 +976,10 @@ struct CudaBackend : Backend {
     void launch_seed_count(const SeedIndexParams& p) override { launch("seed_count", seed_count_kernel, (p.numPos + 255) / 256, 256, 0, p); }
     void launch_seed_fill(const SeedIndexParams& p) override { launch("seed_fill", seed_fill_kernel, (p.numPos + 255) / 256, 256, 0, p); }
     void launch_scan(int* data, int count) override {
+        if (count <= 0) {  // no tiles (a launch of no CTAs is refused): only the total, 0
+            zero(data, sizeof(int));
+            return;
+        }
         const int numTiles = (count + SCAN_TILE - 1) / SCAN_TILE;
         int* tileSums = static_cast<int*>(alloc((size_t)numTiles * sizeof(int)));
         launch("scan", scan_tile_sums_kernel, numTiles, SCAN_THREADS, 0, data, count, tileSums);
@@ -990,14 +994,8 @@ struct CudaBackend : Backend {
         launch("seed_plan", seed_plan_kernel<CAP, THREADS, CoopGroup<GW>>, (p.numReads + GROUPS - 1) / GROUPS, THREADS, smem, p);
     }
     void launch_seed_plan(const SeedPlanParams& p) override {
-        // a read has t + 1 <= min(maxLen / Ls, seedK + 1) seeds: groups of 16 lanes look them all up in one round
-        // when that is at most 16, whole warps otherwise (or when the read lengths are not known)
-        const bool narrow = p.maxLen > 0 && p.Ls > 0 && std::min(p.maxLen / p.Ls, p.seedK + 1) <= 16;
-        with_seed_cap(p.level, [&](auto cap) {
-            constexpr int CAP = decltype(cap)::value;
-            if constexpr (CAP == SEED_CAND_2) launch_seed_plan_t<CAP, 64, 32>(p);  // the last level: a warp per read, two reads per CTA
-            else if (narrow) launch_seed_plan_t<CAP, 128, 16>(p);
-            else launch_seed_plan_t<CAP, 128, 32>(p);
+        with_seed_plan_instance(p, [&](auto cap, auto threads, auto gw) {
+            launch_seed_plan_t<decltype(cap)::value, decltype(threads)::value, decltype(gw)::value>(p);
         });
     }
     void launch_fin_count(const FinParams& p) override { launch("fin_count", fin_count_kernel, (p.numReads + 255) / 256, 256, 0, p); }

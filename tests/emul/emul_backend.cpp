@@ -16,6 +16,7 @@
 #include "eb_core.h"
 #include "eb_dispatch.h"
 #include "eb_engine.h"
+#include "host_coop.h"
 #include "host_warp.h"
 
 namespace ebhost {
@@ -169,8 +170,23 @@ struct EmulBackend : Backend {
         }
         data[count] = run;
     }
+    // Serial planning (one member per read) unless EDLIB_EMUL_SEED_GROUP=device: then the instance the CUDA backend
+    // launches, its groups as lane threads (host_coop.h).
     void launch_seed_plan(const SeedPlanParams& p) override {
         ++launchesCount;
+        const char* mode = getenv("EDLIB_EMUL_SEED_GROUP");
+        if (mode && strcmp(mode, "device") == 0) {
+            with_seed_plan_instance(p, [&](auto cap, auto threads, auto gw) {
+                constexpr int CAP = decltype(cap)::value, THREADS = decltype(threads)::value, GW = decltype(gw)::value;
+                constexpr int GROUPS = 32 / GW;  // per warp
+                std::vector<int> E((size_t)GROUPS * CAP), ctl((size_t)GROUPS * seed_ctl_words(GW));
+                const int ctas = (p.numReads + THREADS / GW - 1) / (THREADS / GW);
+                ebhost::run_lane_groups<GW>(ctas, THREADS, [&](int slot, int g) {
+                    seed_plan_read<CAP, ebhost::CoopThreads<GW>>(p, slot, E.data() + g * CAP, ctl.data() + g * seed_ctl_words(GW));
+                });
+            });
+            return;
+        }
         std::vector<int> E(SEED_CAND_2);
         int ctl[SEED_CTL];
         with_seed_cap(p.level, [&](auto cap) {
