@@ -22,6 +22,8 @@
 
 namespace eb {
 void host_parallel_ranges(size_t n, size_t grain, const std::function<void(size_t, size_t)>& fn);  // eb_engine.cpp
+void free_result_arrays(EdlibAlignResult* results, size_t lo, size_t hi);  // eb_engine.cpp: frees and clears them
+void fail_results(EdlibAlignResult* results, int n);  // eb_engine.cpp: error results (status, distance -1, no arrays)
 Backend* create_backend(std::string* err);  // provided by the backend object linked into this library
 int select_device(int device, std::string* err);  // 0 on success
 }
@@ -100,12 +102,19 @@ SideEngine* side_engine_acquire() {
     return s;
 }
 
-void fail_results(EdlibAlignResult* results, int n) {
-    for (int i = 0; i < n; ++i) {
-        memset(&results[i], 0, sizeof(results[i]));
-        results[i].status = EDLIB_STATUS_ERROR;
-        results[i].editDistance = -1;
-    }
+// the statistics of the last pass of e (its device times are read now)
+void copy_stats(eb::Engine* e, EdlibB200Stats* s) {
+    e->finish_stats();
+    s->kernelMs = e->stats.kernelMs;
+    s->k1Ms = e->stats.k1Ms;
+    s->launches = e->stats.launches;
+    s->h2dBytes = e->stats.h2dBytes;
+    s->d2hBytes = e->stats.d2hBytes;
+    s->k1Cells = e->stats.k1Cells;
+    s->wCells = e->stats.wCells;
+    s->filterDecided = e->stats.filterDecided;
+    s->filterFallback = e->stats.filterFallback;
+    s->filterWindows = (int)std::min<long long>(e->stats.filterWindows, 0x7fffffff);
 }
 
 }  // namespace
@@ -155,7 +164,7 @@ static int align_batch_entry(const char* const* queries, const int* queryLengths
     std::lock_guard<std::mutex> lock(g_mu);
     eb::Engine* e = engine_locked();
     if (!e) {  // no usable device: fail loudly, there is no CPU path
-        fail_results(results, numPairs);
+        eb::fail_results(results, numPairs);
         return EDLIB_STATUS_ERROR;
     }
     t_lastEngine = e;
@@ -307,21 +316,12 @@ EDLIB_API int edlibB200TuneHostAllocator(void) {
 // threads freed themselves.
 EDLIB_API void edlibB200FreeResults(EdlibAlignResult* results, int n) {
     if (!results || n <= 0) return;
-    auto free_range = [results](size_t lo, size_t hi) {
-        for (size_t i = lo; i < hi; ++i) {
-            free(results[i].endLocations);
-            free(results[i].startLocations);
-            free(results[i].alignment);
-            results[i].endLocations = results[i].startLocations = NULL;
-            results[i].alignment = NULL;
-        }
-    };
     if (n < 65536) {
-        free_range(0, (size_t)n);
+        eb::free_result_arrays(results, 0, (size_t)n);
         return;
     }
     std::lock_guard<std::mutex> lock(g_mu);  // the host pool serves one client at a time
-    eb::host_parallel_ranges((size_t)n, 16384, free_range);
+    eb::host_parallel_ranges((size_t)n, 16384, [results](size_t lo, size_t hi) { eb::free_result_arrays(results, lo, hi); });
 }
 
 EDLIB_API int edlibB200Available(void) {
@@ -383,19 +383,7 @@ EDLIB_API int edlibB200BatchCompute(EdlibB200Batch* batch, EdlibB200Stats* stats
         e->lastError = ex.what();
         return EDLIB_STATUS_ERROR;
     }
-    if (statsOut) {
-        e->finish_stats();
-        statsOut->kernelMs = e->stats.kernelMs;
-        statsOut->k1Ms = e->stats.k1Ms;
-        statsOut->launches = e->stats.launches;
-        statsOut->h2dBytes = e->stats.h2dBytes;
-        statsOut->d2hBytes = e->stats.d2hBytes;
-        statsOut->k1Cells = e->stats.k1Cells;
-        statsOut->wCells = e->stats.wCells;
-        statsOut->filterDecided = e->stats.filterDecided;
-        statsOut->filterFallback = e->stats.filterFallback;
-        statsOut->filterWindows = (int)std::min<long long>(e->stats.filterWindows, 0x7fffffff);
-    }
+    if (statsOut) copy_stats(e, statsOut);
     return EDLIB_STATUS_OK;
 }
 
@@ -478,18 +466,7 @@ EDLIB_API void edlibB200LastStats(EdlibB200Stats* s) {
     if (!s) return;
     memset(s, 0, sizeof(*s));
     if (!g_engine || !engine_locked()) return;
-    eb::Engine* e = t_lastEngine ? t_lastEngine : g_engine;  // the engine this thread's last call ran on
-    e->finish_stats();
-    s->kernelMs = e->stats.kernelMs;
-    s->k1Ms = e->stats.k1Ms;
-    s->launches = e->stats.launches;
-    s->h2dBytes = e->stats.h2dBytes;
-    s->d2hBytes = e->stats.d2hBytes;
-    s->k1Cells = e->stats.k1Cells;
-    s->wCells = e->stats.wCells;
-    s->filterDecided = e->stats.filterDecided;
-    s->filterFallback = e->stats.filterFallback;
-    s->filterWindows = (int)std::min<long long>(e->stats.filterWindows, 0x7fffffff);
+    copy_stats(t_lastEngine ? t_lastEngine : g_engine, s);  // the engine this thread's last call ran on
 }
 
 EDLIB_API int edlibB200LastKernelReport(char* buf, int bufLen) {

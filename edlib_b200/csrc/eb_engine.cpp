@@ -123,54 +123,100 @@ static int code_map(const uint32_t (&present)[8], uint8_t (&map)[256], int other
     return ncodes;
 }
 
+// Encodes a target by its own alphabet, in place: `raw` holds its n bytes on the device, zero-padded to round_up(n, 16).
+// Presence set on the device, code map on the host (a byte the target lacks gets the extra code, which matches
+// nothing), encoding on the device.  Returns tc.ncodes.
+static int encode_target(Backend* be, uint8_t* raw, int n, TargetCodes& tc) {
+    std::vector<MaskItem> items;
+    for (int s0 = 0; s0 < n; s0 += 65536) items.push_back(MaskItem{(uint64_t)s0, std::min(65536, n - s0), 0});
+    DevBuf<MaskItem> dItems(be, items.size());
+    dItems.upload(items.data(), items.size());
+    tc.dMask.alloc(be, 8);
+    be->zero(tc.dMask.p, 8 * sizeof(uint32_t));
+    MaskParams mp;
+    memset(&mp, 0, sizeof(mp));
+    mp.raw = raw;
+    mp.items = dItems.p;
+    mp.numItems = (int)items.size();
+    mp.masks = tc.dMask.p;
+    mp.unionSet = -1;
+    be->launch_mask(mp);
+    uint32_t present[8];
+    be->d2h(present, tc.dMask.p, sizeof(present));
+    int distinct = 0;
+    for (int b = 0; b < 256; ++b) distinct += (present[b >> 5] >> (b & 31)) & 1u;
+    uint8_t map[256];
+    code_map(present, map, distinct);
+    tc.dMap.alloc(be, 256);
+    tc.dMap.upload(map, 256);
+    EncodeParams ep{raw, (uint64_t)round_up((size_t)n, 16), tc.dMap.p};
+    be->launch_encode(ep);
+    // no spare code when every byte value occurs in the target: then no read byte is foreign
+    tc.ncodes = distinct >= 256 ? 256 : std::max(1, std::min(distinct, 255));
+    return tc.ncodes;
+}
+
+// The batch object for `in`, with nothing of an earlier batch left in it (staged API: results before compute find
+// none) and the per-pair vectors sized for the caller's pairs.  The spare object of the last batch is reused: its host
+// vectors keep their pages.  On failure the object stays the spare one.
+Prepared* Engine::take_prepared(const BatchInput& in) {
+    if (!spare_) spare_ = new Prepared();
+    Prepared* p = spare_;
+    p->bind(be_);
+    p->tg.clear();
+    p->hasEq = false;
+    p->ncodes = 0;
+    p->computed = false;
+    p->classified = false;
+    p->groups.clear();
+    p->wPairsBase.clear();
+    p->otherPairs.clear();
+    p->ed.clear();
+    p->endStart.clear();
+    p->endCount.clear();
+    p->endPool.clear();
+    p->startPool.clear();
+    p->alnStart.clear();
+    p->alnLen.clear();
+    p->alnPool.clear();
+    p->N = in.numPairs;
+    p->cfg = in.config;
+    p->strands = in.strands;
+    p->strand.clear();
+    p->mode = (in.config.mode == EDLIB_MODE_SHW) ? MODE_SHW : (in.config.mode == EDLIB_MODE_HW) ? MODE_HW : MODE_NW;
+    p->qlen.resize(p->N);
+    p->tlen.resize(p->N);
+    p->tidx.resize(p->N);
+    p->qoff.resize(p->N);
+    spare_ = nullptr;
+    return p;
+}
+
+// After a failure: nothing may still run on the device (staging blocks go back to the cache, buffers to the pool) and
+// no mark stays live.  Never throws.
+void Engine::quiesce() {
+    try {
+        be_->sync_all();
+        be_->release_marks();
+    } catch (...) {
+    }
+}
+
 // ---------------------------------------------------------------------------------------------
 // prepare
 // ---------------------------------------------------------------------------------------------
 Prepared* Engine::prepare(const BatchInput& in) {
     Backend* be = be_;
     Trace trace;
-    // the host vectors of the previous batch are reused (their pages stay mapped)
-    Prepared* p = spare_ ? spare_ : new Prepared();
-    spare_ = nullptr;
+    Prepared* p = take_prepared(in);
     try {
-        p->bind(be);
-        p->tg.clear();
-        p->hasEq = false;
-        p->ncodes = 0;
-        p->computed = false;
-        p->classified = false;
-        // nothing of an earlier batch may survive in the result arrays (staged API: results before compute)
-        p->ed.clear();
-        p->endStart.clear();
-        p->endCount.clear();
-        p->endPool.clear();
-        p->startPool.clear();
-        p->alnStart.clear();
-        p->alnLen.clear();
-        p->alnPool.clear();
-        p->N = in.numPairs;
-        p->cfg = in.config;
-        p->strands = in.strands;
-        p->strand.clear();
-        p->mode = (in.config.mode == EDLIB_MODE_SHW) ? MODE_SHW : (in.config.mode == EDLIB_MODE_HW) ? MODE_HW : MODE_NW;
         int N = p->N;  // the caller's pairs; a strand batch doubles it after packing
-        p->qlen.resize(N);
-        p->tlen.resize(N);
-        p->tidx.resize(N);
-        p->qoff.resize(N);
-        {
-            std::atomic<int> bad(0);
-            parallel_ranges((size_t)N, 65536, [&](size_t lo, size_t hi) {
-                bool b = false;
-                for (size_t i = lo; i < hi; ++i) {
-                    p->qlen[i] = in.queryLengths[i];
-                    p->tlen[i] = in.targetLengths[i];
-                    if (p->qlen[i] < 0 || p->tlen[i] < 0) b = true;
-                }
-                if (b) bad.store(1, std::memory_order_relaxed);
-            });
-            if (bad.load()) throw std::runtime_error("negative sequence length");
-        }
+        if (parallel_any((size_t)N, 65536, [&](size_t i) {
+                p->qlen[i] = in.queryLengths[i];
+                p->tlen[i] = in.targetLengths[i];
+                return p->qlen[i] < 0 || p->tlen[i] < 0;
+            }))
+            throw std::runtime_error("negative sequence length");
 
         // identical (pointer, length) targets are uploaded and encoded once: open-addressing table over the pairs
         // (no node allocations: a batch of 100,000 pairs with their own targets spends ~1 ms here)
@@ -179,20 +225,10 @@ Prepared* Engine::prepare(const BatchInput& in) {
             int len;
             bool operator==(const Key& o) const { return ptr == o.ptr && len == o.len; }
         };
-        bool oneTarget = N > 0;  // the usual batch shape (reads over one shared target), checked in parallel
-        if (N >= 131072) {
-            std::atomic<int> differs(0);
-            const Key first{in.targets[0], in.targetLengths[0]};
-            parallel_ranges((size_t)N, 65536, [&](size_t lo, size_t hi) {
-                bool d = false;
-                for (size_t i = lo; i < hi; ++i)
-                    if (in.targets[i] != first.ptr || in.targetLengths[i] != first.len) d = true;
-                if (d) differs.store(1, std::memory_order_relaxed);
-            });
-            oneTarget = !differs.load();
-        } else {
-            oneTarget = false;
-        }
+        // the usual batch shape (reads over one shared target), checked in parallel
+        const bool oneTarget = N >= 131072 && !parallel_any((size_t)N, 65536, [&](size_t i) {
+            return in.targets[i] != in.targets[0] || in.targetLengths[i] != in.targetLengths[0];
+        });
         if (oneTarget) {
             p->tg.push_back(Target{in.targets[0], in.targetLengths[0], 0});
             parallel_ranges((size_t)N, 65536, [&](size_t lo, size_t hi) {
@@ -268,17 +304,11 @@ Prepared* Engine::prepare(const BatchInput& in) {
             const size_t qBytes = N ? (size_t)(p->qoff[N - 1] + (uint64_t)p->qlen[N - 1]) : 0;
             // Queries that lie back to back in PINNED caller memory (a read array the caller allocated page-locked) go
             // to the device straight from there: no staging copy, no host memory traffic besides the DMA itself.
-            bool direct = false;
-            if (tun.directUpload && N > 0 && qBytes >= tun.directMinBytes) {
-                std::atomic<int> gaps(0);
-                parallel_ranges((size_t)N, 65536, [&](size_t lo, size_t hi) {
-                    bool g = false;
-                    for (size_t i = std::max<size_t>(lo, 1); i < hi; ++i)
-                        if (in.queries[i] != in.queries[i - 1] + p->qlen[i - 1]) g = true;
-                    if (g) gaps.store(1, std::memory_order_relaxed);
-                });
-                direct = !gaps.load() && be->host_pinned(in.queries[0], qBytes);
-            }
+            const bool direct = tun.directUpload && N > 0 && qBytes >= tun.directMinBytes &&
+                                !parallel_any((size_t)N, 65536, [&](size_t i) {
+                                    return i > 0 && in.queries[i] != in.queries[i - 1] + p->qlen[i - 1];
+                                }) &&
+                                be->host_pinned(in.queries[0], qBytes);
             if (direct) be->h2d(p->dSeq.p, in.queries[0], qBytes);
             const int firstItem = direct ? N : 0;
             size_t allBytes = direct ? 0 : qBytes;
@@ -486,10 +516,7 @@ Prepared* Engine::prepare(const BatchInput& in) {
         be->sync();
         trace.mark("prepare: upload+alphabet");
     } catch (...) {
-        try {
-            be->sync_all();  // nothing may still be reading the staging block when it goes back to the cache
-        } catch (...) {
-        }
+        quiesce();  // nothing may still be reading the staging block when it goes back to the cache
         delete p;
         throw;
     }
@@ -498,7 +525,7 @@ Prepared* Engine::prepare(const BatchInput& in) {
 
 // Groups the pairs by (target, word class): a pure function of the lengths, the distinct targets and the
 // config, so prepare() runs it on the host workers while the sequences travel to the device; the lists stay
-// with the batch (and, through the spare batch object, keep their storage from call to call).
+// with the batch (and the per-thread pieces, through the spare batch object, keep their storage from call to call).
 void Engine::classify(Prepared* p) {
     const int N = p->N;
     const int mode = p->mode;
@@ -511,20 +538,16 @@ void Engine::classify(Prepared* p) {
     for (auto& kv : groups) kv.second.clear();
     {
         // contiguous ranges of pairs are classified on a few host threads and concatenated in order
-        const size_t nparts = host_parts((size_t)N, 65536);
         std::vector<Prepared::Part>& parts = p->parts;
-        parts.resize(nparts);
-        for (auto& P : parts) {
+        parts.resize(HostPool::get().width());
+        const size_t nparts = parallel_parts((size_t)N, 65536, [&](size_t t, size_t lo, size_t hi) {
+            Prepared::Part& P = parts[t];
             for (auto& kv : P.groups) kv.second.clear();
             P.wPairs.clear();
             P.other.clear();
-        }
-        auto classify = [&](size_t t) {
-            Prepared::Part& P = parts[t];
             std::pair<int, int> lastKey(-1, -1);
             std::vector<int>* lastList = nullptr;
-            const int lo = (int)((size_t)N * t / nparts), hi = (int)((size_t)N * (t + 1) / nparts);
-            for (int i = lo; i < hi; ++i) {
+            for (int i = (int)lo; i < (int)hi; ++i) {
                 const int m = p->qlen[i], n = p->tlen[i];
                 p->special[i] = (m == 0 || n == 0) ? 1 : 0;
                 if (p->special[i] || (mode == MODE_NW && k >= 0 && k < abs(n - m))) {  // ref cpp:166-184, 744
@@ -536,16 +559,16 @@ void Engine::classify(Prepared* p) {
                     if (key != lastKey) {  // neighbours usually share their group
                         lastKey = key;
                         lastList = &P.groups[key];
-                        if (lastList->empty()) lastList->reserve((size_t)(hi - i));
+                        if (lastList->empty()) lastList->reserve(hi - (size_t)i);
                     }
                     lastList->push_back(i);
                 } else {
                     P.wPairs.push_back(i);
                 }
             }
-        };
-        HostPool::get().run(nparts, classify);
-        for (Prepared::Part& P : parts) {
+        });
+        for (size_t t = 0; t < nparts; ++t) {
+            const Prepared::Part& P = parts[t];
             for (auto& kv : P.groups) {
                 if (kv.second.empty()) continue;
                 std::vector<int>& dst = groups[kv.first];
@@ -635,10 +658,7 @@ void Engine::compute(Prepared* p) {
     }
     // ---- device-driven first seed level of every group that may take it: enqueued without waiting --------
     if (devSlices > 0) {
-        ps.dev_begin(devSlices);
-        ps.dPool.alloc(be, (size_t)(4 * devReads + devReads / 4 + (long long)DEV_EXTRA_SLACK * devSlices + 64));
-        ps.dLists.alloc(be, (size_t)devListed);
-        p->endPool.resize(ps.dPool.n);
+        ps.dev_begin(devReads, devSlices, devListed);
         for (Route& r : routes) {
             if (!r.device) continue;
             const std::vector<int>& list = *r.list;
@@ -658,7 +678,7 @@ void Engine::compute(Prepared* p) {
                 ps.dev_enqueue_slice(r.t, r.nw, consecutive ? list.front() : -1, list.data(), first,
                                      std::min(sliceReads, (int)list.size() - first));
         }
-        p->endPool.resize((size_t)ps.poolReserved);  // what the slices were actually handed
+        ps.dev_enqueued();
         trace.mark("compute: device stage enqueued");
     } else {
         ps.host_touch_all();
@@ -761,8 +781,8 @@ static bool materialize_one(const Prepared* p, int i, EdlibAlignResult& r) {
     return true;
 }
 
-static void free_result_arrays(EdlibAlignResult* results, int n) {
-    for (int i = 0; i < n; ++i) {
+void free_result_arrays(EdlibAlignResult* results, size_t lo, size_t hi) {
+    for (size_t i = lo; i < hi; ++i) {
         free(results[i].endLocations);
         free(results[i].startLocations);
         free(results[i].alignment);
@@ -771,19 +791,26 @@ static void free_result_arrays(EdlibAlignResult* results, int n) {
     }
 }
 
-void Engine::materialize(Prepared* p, EdlibAlignResult* results) {
+void fail_results(EdlibAlignResult* results, int n) {
+    for (int i = 0; i < n; ++i) {
+        memset(&results[i], 0, sizeof(results[i]));
+        results[i].status = EDLIB_STATUS_ERROR;
+        results[i].editDistance = -1;
+    }
+}
+
+void Engine::materialize(Prepared* p, EdlibAlignResult* results, const std::vector<int>* list) {
     if (!p->computed) throw std::runtime_error("results requested from a batch that was not (successfully) computed");
     Trace trace;
     const int N = p->strands ? p->N / 2 : p->N;  // a strand batch: one result per read, from its winning strand
-    std::atomic<int> failed(0);
-    parallel_ranges((size_t)N, 65536, [&](size_t lo, size_t hi) {
-        for (int i = (int)lo; i < (int)hi; ++i) {
-            const int pair = p->strands ? 2 * i + p->strand[i] : i;
-            if (!materialize_one(p, pair, results[i])) failed.store(1, std::memory_order_relaxed);
-        }
+    const size_t n = list ? list->size() : (size_t)N;
+    auto result_of = [&](size_t j) { return list ? (*list)[j] : (int)j; };
+    const bool failed = parallel_any(n, list ? 4096 : 65536, [&](size_t j) {
+        const int i = result_of(j);
+        return !materialize_one(p, p->strands ? 2 * i + p->strand[i] : i, results[i]);
     });
-    if (failed.load()) {
-        free_result_arrays(results, N);
+    if (failed) {  // every listed result was written: all of them give their arrays back
+        for (size_t j = 0; j < n; ++j) free_result_arrays(results, (size_t)result_of(j), (size_t)result_of(j) + 1);
         throw std::runtime_error("out of memory while building the results");
     }
     trace.mark("materialize");
@@ -832,39 +859,12 @@ TargetHandle* Engine::target_prepare(const char* target, int n) {
             h->codes.upload(stage.p, h->bytes);
             be->sync();
         }
-        std::vector<MaskItem> items;
-        for (int s0 = 0; s0 < n; s0 += 65536) items.push_back(MaskItem{(uint64_t)s0, std::min(65536, n - s0), 0});
-        DevBuf<MaskItem> dItems(be, items.size());
-        dItems.upload(items.data(), items.size());
-        h->dMask.alloc(be, 8);
-        be->zero(h->dMask.p, 8 * sizeof(uint32_t));
-        MaskParams mp;
-        memset(&mp, 0, sizeof(mp));
-        mp.raw = h->codes.p;
-        mp.items = dItems.p;
-        mp.numItems = (int)items.size();
-        mp.masks = h->dMask.p;
-        mp.unionSet = -1;
-        be->launch_mask(mp);
-        be->d2h(h->tmask, h->dMask.p, sizeof(h->tmask));
-        int ncodes = 0;
-        for (int b = 0; b < 256; ++b) ncodes += (h->tmask[b >> 5] >> (b & 31)) & 1u;
-        code_map(h->tmask, h->map, ncodes);
-        h->ncodesRaw = ncodes;
-        h->dMap.alloc(be, 256);
-        h->dMap.upload(h->map, 256);
-        EncodeParams ep{h->codes.p, (uint64_t)round_up((size_t)n, 16), h->dMap.p};
-        be->launch_encode(ep);
-        const int codes = ncodes >= 256 ? 256 : std::max(1, std::min(ncodes, 255));
-        build_seed_index(be, tun, h->idx, h->codes.p, n, codes);
+        build_seed_index(be, tun, h->idx, h->codes.p, n, encode_target(be, h->codes.p, n, h->tc));
         be->sync();
         targets_.push_back(h);
         return h;
     } catch (...) {
-        try {
-            be->sync_all();
-        } catch (...) {
-        }
+        quiesce();
         delete h;
         throw;
     }
@@ -891,30 +891,19 @@ int Engine::align_batch(const BatchInput& in, EdlibAlignResult* results, unsigne
     Prepared* p = nullptr;
     stats = EngineStats();
     statsPending_ = false;
-    bool built = false;  // results[] holds malloc'd arrays
     try {
         if (align_streamed(in, results)) return EDLIB_STATUS_OK;
         p = prepare(in);
         compute(p);
-        built = true;
         materialize(p, results);  // releases what it built when it fails
         if (strands) strands_of(p, strands);
         release(p);
         return EDLIB_STATUS_OK;
     } catch (const std::exception& e) {
         lastError = e.what();
-        try {
-            be_->sync_all();
-            be_->release_marks();
-        } catch (...) {
-        }
+        quiesce();
         if (p) release(p);
-        (void)built;
-        for (int i = 0; i < in.numPairs; ++i) {
-            memset(&results[i], 0, sizeof(results[i]));
-            results[i].status = EDLIB_STATUS_ERROR;
-            results[i].editDistance = -1;
-        }
+        fail_results(results, in.numPairs);
         return EDLIB_STATUS_ERROR;
     }
 }
@@ -968,11 +957,12 @@ bool Engine::align_streamed(const BatchInput& in, EdlibAlignResult* results) {
         bool differs = false;
         bool gaps = false;  // some query does not start where its predecessor ends (in the caller's memory)
     };
-    const size_t nparts = host_parts((size_t)N, 32768);
-    std::vector<Scan> scans(nparts);
-    HostPool::get().run(nparts, [&](size_t t) {
+    // the scan and the offset pass below cut the pairs into the same parts: the offsets start from the scan's byte sums
+    auto over_parts = [N](const std::function<void(size_t, size_t, size_t)>& fn) { return parallel_parts((size_t)N, 32768, fn); };
+    std::vector<Scan> scans(HostPool::get().width());
+    const size_t nparts = over_parts([&](size_t t, size_t lo, size_t hi) {
         Scan s;
-        for (size_t i = (size_t)N * t / nparts, hi = (size_t)N * (t + 1) / nparts; i < hi; ++i) {
+        for (size_t i = lo; i < hi; ++i) {
             if (in.targets[i] != tptr || in.targetLengths[i] != n) s.differs = true;
             if (i > 0 && in.queries[i] != in.queries[i - 1] + in.queryLengths[i - 1]) s.gaps = true;
             const int m = in.queryLengths[i];
@@ -982,6 +972,7 @@ bool Engine::align_streamed(const BatchInput& in, EdlibAlignResult* results) {
         }
         scans[t] = s;
     });
+    scans.resize(nparts);
     Scan all;
     for (const Scan& s : scans) {
         all.differs |= s.differs;
@@ -996,28 +987,21 @@ bool Engine::align_streamed(const BatchInput& in, EdlibAlignResult* results) {
     if (all.bytes + n > (1LL << 31) - (1 << 20)) return false;
 
     Trace trace;
-    Prepared* p = spare_ ? spare_ : new Prepared();
-    spare_ = nullptr;
+    Prepared* p = take_prepared(in);
     StreamJob job;
     bool poolBusy = false;
+    auto stop_workers = [&]() {
+        if (!poolBusy) return;
+        poolBusy = false;
+        {
+            std::lock_guard<std::mutex> lock(job.mu);
+            job.abort = true;
+            job.cv.notify_all();
+        }
+        HostPool::get().end(true);
+    };
     std::function<void()> freeBuilt;
     try {
-        p->bind(be);
-        p->tg.clear();
-        p->hasEq = false;
-        p->computed = false;
-        p->classified = false;
-        p->groups.clear();
-        p->wPairsBase.clear();
-        p->otherPairs.clear();
-        p->N = N;
-        p->cfg = in.config;
-        p->strands = false;
-        p->mode = MODE_HW;
-        p->qlen.resize(N);
-        p->tlen.resize(N);
-        p->tidx.resize(N);
-        p->qoff.resize(N);
         p->special.resize(N);
         p->alphaLen.resize(N);
         reset_results(p);
@@ -1027,9 +1011,9 @@ bool Engine::align_streamed(const BatchInput& in, EdlibAlignResult* results) {
         HostBuf<int> hQlen(be, (size_t)N);
         std::vector<long long> partOff(nparts + 1, 0);
         for (size_t t = 0; t < nparts; ++t) partOff[t + 1] = partOff[t] + scans[t].bytes;
-        HostPool::get().run(nparts, [&](size_t t) {
+        over_parts([&](size_t t, size_t lo, size_t hi) {
             uint64_t off = (uint64_t)partOff[t];
-            for (size_t i = (size_t)N * t / nparts, hi = (size_t)N * (t + 1) / nparts; i < hi; ++i) {
+            for (size_t i = lo; i < hi; ++i) {
                 const int m = in.queryLengths[i];
                 p->qlen[i] = m;
                 p->tlen[i] = n;
@@ -1052,7 +1036,6 @@ bool Engine::align_streamed(const BatchInput& in, EdlibAlignResult* results) {
         p->dQoff.alloc(be, N);
         p->dQlen.alloc(be, N);
         DevBuf<int> dAlpha(be, (size_t)N);
-        stats.h2dBytes += (long long)total + 12LL * N;
         trace.mark("stream: lengths + offsets + buffers");
 
         // slices of reads; every slice is packed by all workers together (parts), so that slice 0 is on its way first
@@ -1066,16 +1049,21 @@ bool Engine::align_streamed(const BatchInput& in, EdlibAlignResult* results) {
         job.partsLeft.assign((size_t)numSlices, partsPerSlice);
         job.resultsReady.assign((size_t)numSlices, 0);
         const bool matInJob = in.config.task == EDLIB_TASK_DISTANCE;
-        const int matPartsPerSlice = partsPerSlice;
         const uint64_t allocated = be->mark(Backend::STREAM_COMPUTE);  // the copy stream may use the buffers after this
         be->wait(Backend::STREAM_COPY, allocated);
 
-        auto slice_lo = [&](int s) { return (int)std::min<long long>((long long)s * sliceReads, N); };
+        // Reads [first, end) of part `part` of slice s, or of the whole slice (part < 0).  Packing, uploads and result
+        // structs cut the slices alike; the error path uses it after this scope is gone, so it holds copies.
+        const auto part_range = [N, sliceReads, partsPerSlice](int s, int part) {
+            const int lo = (int)std::min<long long>((long long)s * sliceReads, N);
+            const int hi = (int)std::min<long long>((long long)(s + 1) * sliceReads, N);
+            if (part < 0) return std::make_pair(lo, hi);
+            return std::make_pair(lo + (int)((long long)(hi - lo) * part / partsPerSlice),
+                                  lo + (int)((long long)(hi - lo) * (part + 1) / partsPerSlice));
+        };
         auto pack_part = [&](size_t task) {
-            const int s = (int)(task / (size_t)partsPerSlice), part = (int)(task % (size_t)partsPerSlice);
-            const int lo = slice_lo(s), hi = slice_lo(s + 1);
-            const int a = lo + (int)((long long)(hi - lo) * part / partsPerSlice);
-            const int b = lo + (int)((long long)(hi - lo) * (part + 1) / partsPerSlice);
+            const int s = (int)(task / (size_t)partsPerSlice);
+            const auto [a, b] = part_range(s, (int)(task % (size_t)partsPerSlice));
             if (b > a) {
                 const size_t off = (size_t)p->qoff[a];
                 const size_t bytes = (size_t)(p->qoff[b - 1] + (uint64_t)p->qlen[b - 1]) - off;
@@ -1110,15 +1098,13 @@ bool Engine::align_streamed(const BatchInput& in, EdlibAlignResult* results) {
             }
         };
         auto mat_part = [&](size_t task) {
-            const int s = (int)(task / (size_t)matPartsPerSlice), part = (int)(task % (size_t)matPartsPerSlice);
+            const int s = (int)(task / (size_t)partsPerSlice);
             {
                 std::unique_lock<std::mutex> lock(job.mu);
                 job.cv.wait(lock, [&]() { return job.resultsReady[(size_t)s] || job.abort; });
                 if (job.abort) return;
             }
-            const int lo = slice_lo(s), hi = slice_lo(s + 1);
-            const int a = lo + (int)((long long)(hi - lo) * part / matPartsPerSlice);
-            const int b = lo + (int)((long long)(hi - lo) * (part + 1) / matPartsPerSlice);
+            const auto [a, b] = part_range(s, (int)(task % (size_t)partsPerSlice));
             for (int i = a; i < b; ++i) {
                 if (p->ed[i] == -2) continue;  // pending: the host-driven stages will settle it
                 if (!materialize_one(p, i, results[i])) job.failed.store(1, std::memory_order_relaxed);
@@ -1128,18 +1114,14 @@ bool Engine::align_streamed(const BatchInput& in, EdlibAlignResult* results) {
         // direct uploads need no packing: the orchestrator issues the copies of every slice itself, slice by slice, so
         // that they reach the copy stream in the order the slices are computed in
         const size_t packTasks = direct ? 0 : (size_t)numSlices * partsPerSlice;
-        const size_t matTasks = matInJob ? (size_t)numSlices * matPartsPerSlice : 0;
+        const size_t matTasks = matInJob ? (size_t)numSlices * partsPerSlice : 0;
         job.matDone.assign(matTasks, 0);
-        freeBuilt = [&, sliceReads, matPartsPerSlice]() {  // error path: the arrays of the result structs built so far
+        freeBuilt = [&, part_range, partsPerSlice]() {  // error path: the arrays of the result structs built so far
             for (size_t task = 0; task < job.matDone.size(); ++task) {
                 if (!job.matDone[task]) continue;
-                const int s = (int)(task / (size_t)matPartsPerSlice), part = (int)(task % (size_t)matPartsPerSlice);
-                const int lo = (int)std::min<long long>((long long)s * sliceReads, N);
-                const int hi = (int)std::min<long long>((long long)(s + 1) * sliceReads, N);
-                const int a = lo + (int)((long long)(hi - lo) * part / matPartsPerSlice);
-                const int b = lo + (int)((long long)(hi - lo) * (part + 1) / matPartsPerSlice);
+                const auto [a, b] = part_range((int)(task / (size_t)partsPerSlice), (int)(task % (size_t)partsPerSlice));
                 for (int i = a; i < b; ++i)
-                    if (p->ed[i] != -2) free_result_arrays(results + i, 1);
+                    if (p->ed[i] != -2) free_result_arrays(results, (size_t)i, (size_t)i + 1);
             }
         };
         const std::function<void(size_t)> workerFn = [&](size_t) {
@@ -1174,7 +1156,7 @@ bool Engine::align_streamed(const BatchInput& in, EdlibAlignResult* results) {
         auto issue_direct_uploads = [&]() {
             if (!direct) return;
             for (int s = 0; s < numSlices; ++s) {
-                const int lo = slice_lo(s), hi = slice_lo(s + 1);
+                const auto [lo, hi] = part_range(s, -1);
                 const size_t off = (size_t)p->qoff[lo];
                 const size_t bytes = (size_t)(p->qoff[hi - 1] + (uint64_t)p->qlen[hi - 1]) - off;
                 be->h2d_copy(p->dSeq.p + off, reinterpret_cast<const uint8_t*>(in.queries[0]) + off, bytes);
@@ -1185,22 +1167,13 @@ bool Engine::align_streamed(const BatchInput& in, EdlibAlignResult* results) {
             }
         };
         TargetHandle* const kept = find_target(tptr, n);
-        DevBuf<MaskItem> dItems;
-        DevBuf<uint32_t> dMaskOwn;
-        DevBuf<uint8_t> dMapOwn;
-        const uint32_t* dMaskP = nullptr;
-        const uint8_t* dMapP = nullptr;
-        uint8_t map[256];
-        int ncodes = 0;
+        TargetCodes ownCodes;
+        const TargetCodes& tc = kept ? kept->tc : ownCodes;
         if (kept) {
             if (tOff > qBytes) be->zero(p->dSeq.p + qBytes, tOff - qBytes);
             be->d2d(p->dSeq.p + tOff, kept->codes.p, kept->bytes);  // (bytes == total - tOff)
             job.targetIssued.store(1, std::memory_order_release);
             issue_direct_uploads();
-            dMaskP = kept->dMask.p;
-            dMapP = kept->dMap.p;
-            memcpy(map, kept->map, sizeof(map));
-            ncodes = kept->ncodesRaw;
         } else {
             if (tun.directUpload && be->host_pinned(tptr, (size_t)n)) {  // pinned caller memory: no staging copy
                 be->h2d_copy(p->dSeq.p + tOff, tptr, (size_t)n);
@@ -1216,37 +1189,9 @@ bool Engine::align_streamed(const BatchInput& in, EdlibAlignResult* results) {
             job.targetIssued.store(1, std::memory_order_release);
             issue_direct_uploads();
             be->wait(Backend::STREAM_COMPUTE, targetUp);
-            std::vector<MaskItem> items;
-            for (int s0 = 0; s0 < n; s0 += 65536) items.push_back(MaskItem{(uint64_t)tOff + (uint64_t)s0, std::min(65536, n - s0), 0});
-            dItems.alloc(be, items.size());
-            dItems.upload(items.data(), items.size());
-            dMaskOwn.alloc(be, 8);
-            be->zero(dMaskOwn.p, 8 * sizeof(uint32_t));
-            {
-                MaskParams mp;
-                memset(&mp, 0, sizeof(mp));
-                mp.raw = p->dSeq.p;
-                mp.items = dItems.p;
-                mp.numItems = (int)items.size();
-                mp.masks = dMaskOwn.p;
-                mp.unionSet = -1;
-                be->launch_mask(mp);
-            }
-            uint32_t tmask[8];
-            be->d2h(tmask, dMaskOwn.p, sizeof(tmask));
-            for (int b = 0; b < 256; ++b) ncodes += (tmask[b >> 5] >> (b & 31)) & 1u;
-            code_map(tmask, map, ncodes);  // bytes the target does not hold: the extra code `ncodes`
-            dMapOwn.alloc(be, 256);
-            dMapOwn.upload(map, 256);
-            EncodeParams ep{p->dSeq.p + tOff, (uint64_t)round_up((size_t)n, 16), dMapOwn.p};
-            be->launch_encode(ep);
-            dMaskP = dMaskOwn.p;
-            dMapP = dMapOwn.p;
+            encode_target(be, p->dSeq.p + tOff, n, ownCodes);
         }
-        p->ncodes = std::max(1, std::min(ncodes, 255));
-        if (ncodes >= 256) {  // no spare code: every byte value occurs in the target, so no read byte is foreign
-            p->ncodes = 256;
-        }
+        p->ncodes = tc.ncodes;
         trace.mark("stream: target uploaded + encoded");
         stats = EngineStats();
         stats.h2dBytes = (long long)(kept ? qBytes : total) + 12LL * N;
@@ -1260,15 +1205,7 @@ bool Engine::align_streamed(const BatchInput& in, EdlibAlignResult* results) {
         be->k1_shape(nw, p->ncodes, N, &bt, &rc);
         if (rc <= 0 || !ps.dev_eligible(0, nw) || !ps.seed_index(0) || ps.seedIdx->Ls[0] <= 0) {
             // cannot happen for the batches admitted above except with an exotic alphabet: back to the grouped path
-            if (poolBusy) {
-                {
-                    std::lock_guard<std::mutex> lock(job.mu);
-                    job.abort = true;
-                    job.cv.notify_all();
-                }
-                HostPool::get().end(true);
-                poolBusy = false;
-            }
+            stop_workers();
             be->sync_all();
             be->release_marks();
             release(p);
@@ -1276,9 +1213,7 @@ bool Engine::align_streamed(const BatchInput& in, EdlibAlignResult* results) {
         }
         stats.k1Cells = all.bytes * (long long)n;
         trace.mark("stream: pass + index");
-        ps.dev_begin(numSlices);
-        ps.dPool.alloc(be, (size_t)(4LL * N + N / 4 + (long long)DEV_EXTRA_SLACK * numSlices + 64));
-        p->endPool.resize(ps.dPool.n);
+        ps.dev_begin(N, numSlices, 0);
         trace.mark("stream: target + index");
 
         // ---- slices: enqueue as their uploads are issued ----
@@ -1294,7 +1229,7 @@ bool Engine::align_streamed(const BatchInput& in, EdlibAlignResult* results) {
                 up = job.uploadMark[(size_t)s];
             }
             be->wait(Backend::STREAM_COMPUTE, up);
-            const int lo = slice_lo(s), hi = slice_lo(s + 1);
+            const auto [lo, hi] = part_range(s, -1);
             QAlphaParams qa;
             memset(&qa, 0, sizeof(qa));
             qa.raw = p->dSeq.p;
@@ -1302,11 +1237,11 @@ bool Engine::align_streamed(const BatchInput& in, EdlibAlignResult* results) {
             qa.qlen = p->dQlen.p;
             qa.firstPair = lo;
             qa.numQueries = hi - lo;
-            qa.tmask = dMaskP;
+            qa.tmask = tc.dMask.p;
             qa.alphaLen = dAlpha.p;
             be->launch_qalpha(qa);
             const uint64_t b0 = p->qoff[lo], b1 = p->qoff[hi - 1] + (uint64_t)p->qlen[hi - 1];
-            EncodeParams ep{p->dSeq.p + b0, b1 - b0, dMapP};
+            EncodeParams ep{p->dSeq.p + b0, b1 - b0, tc.dMap.p};
             be->launch_encode(ep);
             ps.extraCopyDst = p->alphaLen.data() + lo;
             ps.extraCopySrc = dAlpha.p + lo;
@@ -1314,7 +1249,7 @@ bool Engine::align_streamed(const BatchInput& in, EdlibAlignResult* results) {
             ps.dev_enqueue_slice(0, nw, 0, nullptr, lo, hi - lo);
             ps.extraCopyBytes = 0;
         }
-        p->endPool.resize((size_t)ps.poolReserved);
+        ps.dev_enqueued();
         trace.mark("stream: slices enqueued");
         // ---- results of the slices as they arrive: released to the workers ----
         for (int s = 0; s < numSlices; ++s) {
@@ -1341,37 +1276,16 @@ bool Engine::align_streamed(const BatchInput& in, EdlibAlignResult* results) {
         stats.launches = be->launches();
         statsPending_ = true;
         p->computed = true;
-        if (matInJob) {
-            std::atomic<int> failed(0);
-            const std::vector<int>& hp = ps.hostPairs;
-            parallel_ranges(hp.size(), 4096, [&](size_t lo, size_t hi) {
-                for (size_t j = lo; j < hi; ++j)
-                    if (!materialize_one(p, hp[j], results[hp[j]])) failed.store(1, std::memory_order_relaxed);
-            });
-            if (failed.load()) throw std::runtime_error("out of memory while building the results");
-        } else {
-            materialize(p, results);
-        }
+        materialize(p, results, matInJob ? &ps.hostPairs : nullptr);  // the slices' result structs are built
         trace.mark("stream: leftovers + results");
         release(p);
         return true;
     } catch (...) {
-        if (poolBusy) {
-            {
-                std::lock_guard<std::mutex> lock(job.mu);
-                job.abort = true;
-                job.cv.notify_all();
-            }
-            try {
-                HostPool::get().end(true);
-            } catch (...) {
-            }
-        }
         try {
-            be->sync_all();
-            be->release_marks();
+            stop_workers();
         } catch (...) {
         }
+        quiesce();
         // result structs built so far own malloc'd arrays: give them back before the caller's array is reset
         // (entries never written are untouched caller memory: only finished result-struct tasks count)
         if (freeBuilt) freeBuilt();

@@ -176,7 +176,8 @@ public:
     // Staged form (bench "inputs resident in HBM" measurement, multi-GPU shards):
     Prepared* prepare(const BatchInput& in);                 // upload, alphabet, encode
     void compute(Prepared* p);                               // every kernel; records come back to the host
-    void materialize(Prepared* p, EdlibAlignResult* results);  // malloc the per-pair arrays
+    // malloc the per-pair arrays, of every result or of the `list`ed ones
+    void materialize(Prepared* p, EdlibAlignResult* results, const std::vector<int>* list = nullptr);
     void release(Prepared* p);
     void classify(Prepared* p);                              // pairs -> (target, word class) groups (host only)
     // One-shot streamed path for large HW batches of short reads over one shared target (eb_engine.cpp): returns
@@ -199,6 +200,8 @@ private:
     Prepared* spare_ = nullptr;  // released batch object whose host vectors the next prepare() reuses
     std::vector<TargetHandle*> targets_;
     TargetHandle* find_target(const char* ptr, int n) const;
+    Prepared* take_prepared(const BatchInput& in);  // a batch object reset for `in` (prepare, align_streamed)
+    void quiesce();  // error paths: wait for the device, release the marks; never throws
     bool statsPending_ = false;
 };
 

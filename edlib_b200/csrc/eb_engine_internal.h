@@ -193,6 +193,28 @@ void parallel_ranges(size_t n, size_t grain, F fn) {
     HostPool::get().run(nthr, [&](size_t t) { fn(n * t / nthr, n * (t + 1) / nthr); });
 }
 
+// fn(part, begin, end) over the host_parts(n, grain) parts of [0, n) (one empty part when n == 0), on the host workers.
+// Returns the number of parts: at most HostPool::get().width(), and the same for the same n and grain.
+template <class F>
+size_t parallel_parts(size_t n, size_t grain, F fn) {
+    const size_t nparts = host_parts(n, grain);
+    HostPool::get().run(nparts, [&](size_t t) { fn(t, n * t / nparts, n * (t + 1) / nparts); });
+    return nparts;
+}
+
+// Whether pred(i) holds for some i in [0, n), on the host workers.  pred is called on every item (no early exit), so it
+// may also write what item i needs.
+template <class P>
+bool parallel_any(size_t n, size_t grain, P pred) {
+    std::atomic<int> any(0);
+    parallel_ranges(n, grain, [&](size_t lo, size_t hi) {
+        bool a = false;
+        for (size_t i = lo; i < hi; ++i) a |= pred(i);
+        if (a) any.store(1, std::memory_order_relaxed);
+    });
+    return any.load() != 0;
+}
+
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 inline size_t round_up(size_t a, size_t b) { return (a + b - 1) / b * b; }
 
@@ -450,18 +472,22 @@ struct SeedIndex {
 // Builds the radix seed index of an encoded target (seed lengths per level, bucket table, positions).
 bool build_seed_index(Backend* be, const EngineTunables& tun, SeedIndex& sx, const uint8_t* tcodes, int n, int ncodes);
 
+// The codes of a target encoded by its own alphabet (encode_target, eb_engine.cpp): dense codes of its bytes in ascending
+// order, every byte it lacks one extra code that matches nothing.
+struct TargetCodes {
+    DevBuf<uint32_t> dMask;    // [8] presence set
+    DevBuf<uint8_t> dMap;      // [256] byte -> code
+    int ncodes = 0;            // codes the kernels see: the extra one included, 256 when every byte value occurs
+};
+
 // A target kept resident on the device (streamed read-set path): its encoded bytes with the padding the kernels rely on,
-// the presence set / code map the encoding came from, and its seed index.
+// its codes and its seed index.
 struct TargetHandle {
     const char* ptr = nullptr;
     int n = 0;
     size_t bytes = 0;          // round_up(n, 16) + 32 encoded bytes (zero padding)
     DevBuf<uint8_t> codes;
-    DevBuf<uint32_t> dMask;    // [8] presence set
-    DevBuf<uint8_t> dMap;      // [256] byte -> code
-    uint32_t tmask[8];
-    uint8_t map[256];
-    int ncodesRaw = 0;         // distinct bytes of the target
+    TargetCodes tc;
     SeedIndex idx;
 };
 
@@ -494,6 +520,8 @@ struct WinRecords {
 // header {end locations, reads pending, pool overflow, windows}.
 // Room of a slice's extra list (end columns beyond the KPOS inline ones of a read) beyond a quarter of its reads.
 constexpr int DEV_EXTRA_SLACK = 16384;
+// Ints of the end-location pool a slice of `count` reads may fill: <= KPOS inline end columns per read + its extra list.
+inline long long dev_slice_pool(long long count) { return 4 * count + count / 4 + DEV_EXTRA_SLACK; }
 struct DevSlice {
     int t = 0, nw = 0;
     int firstPair = -1;      // >= 0: consecutive pairs (no read list on the device)
@@ -675,9 +703,11 @@ struct Pass {
     // ---- device-driven first seed level ----------------------------------------------------------------
     // May group (t, nw) take it?  (HW over a long target, plain equality, seed stage enabled, index available.)
     bool dev_eligible(int t, int nw);
-    // Device arrays of the pass (per-pair results, leftover list, headers); `maxSlices` bounds the slices to come.
-    // (dPool / dLists and the host result arrays are sized by the caller, who knows the reads to come.)
-    void dev_begin(int maxSlices);
+    // Device arrays of the pass (per-pair results, leftover list, headers, end-location pool, read lists) for at most
+    // `maxSlices` slices of `reads` reads in all, `listed` of them in slices of scattered pairs; p->endPool sized to match.
+    void dev_begin(long long reads, int maxSlices, long long listed);
+    // After the last slice is enqueued: p->endPool trimmed to the regions the slices were handed.
+    void dev_enqueued() { p->endPool.resize((size_t)poolReserved); }
     // Enqueues, without any host synchronisation, the whole first level for reads [first, first+count) of a group:
     // seed planning, window sweeps, reduction, assembly of distances and end locations into the slice's pool region.
     // Returns the slice index.

@@ -381,17 +381,10 @@ void Pass::window_outcomes(LaneGroup& c, const std::vector<int>& cand, const int
         long long decided = 0, positions = 0;
         int nSat = 0, nLong = 0;
     };
-    std::vector<Part> parts;
-    std::vector<size_t> partLo;
-    {
-        const size_t nparts = host_parts((size_t)g, 65536);
-        parts.resize(nparts);
-        for (size_t t2 = 0; t2 <= nparts; ++t2) partLo.push_back((size_t)g * t2 / nparts);
-    }
-    auto for_parts = [&](const std::function<void(size_t)>& fn) { HostPool::get().run(parts.size(), fn); };
-    for_parts([&](size_t t2) {
+    std::vector<Part> parts(HostPool::get().width());
+    parts.resize(parallel_parts((size_t)g, 65536, [&](size_t t2, size_t lo, size_t hi) {
         Part& P = parts[t2];
-        for (size_t i = partLo[t2]; i < partLo[t2 + 1]; ++i) {
+        for (size_t i = lo; i < hi; ++i) {
             const int s = cand[i], pair = list[s];
             const Rec& r = out[i];
             if (thr[i] < 0) {
@@ -415,7 +408,7 @@ void Pass::window_outcomes(LaneGroup& c, const std::vector<int>& cand, const int
                 c.repeat[s] = 1;  // too many seed occurrences for this level
             }
         }
-    });
+    }));
     std::vector<long long> partPos(parts.size());
     {
         long long at = (long long)posPool.size();
@@ -430,9 +423,9 @@ void Pass::window_outcomes(LaneGroup& c, const std::vector<int>& cand, const int
         }
         posPool.resize((size_t)at);
     }
-    for_parts([&](size_t t2) {
+    parallel_parts((size_t)g, 65536, [&](size_t t2, size_t lo, size_t hi) {
         long long at = partPos[t2];
-        for (size_t i = partLo[t2]; i < partLo[t2 + 1]; ++i) {
+        for (size_t i = lo; i < hi; ++i) {
             const Rec& r = out[i];
             if (thr[i] < 0 || r.rsv != SEED_WINDOWS) continue;
             const int pair = list[cand[i]];
@@ -759,7 +752,7 @@ bool Pass::dev_eligible(int t, int nw) {
     return true;
 }
 
-void Pass::dev_begin(int maxSlices) {
+void Pass::dev_begin(long long reads, int maxSlices, long long listed) {
     devMode = true;
     dEd.alloc(be, (size_t)N);
     dEndCount.alloc(be, (size_t)N);
@@ -773,6 +766,10 @@ void Pass::dev_begin(int maxSlices) {
     slices.clear();
     slices.reserve((size_t)maxSlices);
     poolReserved = 0;
+    // the pools of any maxSlices slices of `reads` reads in all: their quarters, rounded down, add up to at most a quarter
+    dPool.alloc(be, (size_t)(dev_slice_pool(reads) + (long long)DEV_EXTRA_SLACK * (maxSlices - 1) + 64));
+    if (listed > 0) dLists.alloc(be, (size_t)listed);
+    p->endPool.resize(dPool.n);
 }
 
 int Pass::dev_enqueue_slice(int t, int nw, int firstPair, const int* listHost, int first, int count) {
@@ -785,7 +782,7 @@ int Pass::dev_enqueue_slice(int t, int nw, int firstPair, const int* listHost, i
     sl.firstPair = firstPair >= 0 ? firstPair + first : -1;
     sl.count = count;
     sl.poolBase = poolReserved;
-    sl.poolCap = 4 * count + count / 4 + DEV_EXTRA_SLACK;  // <= KPOS inline positions per read + the slice's extra list
+    sl.poolCap = (int)dev_slice_pool(count);
     poolReserved += sl.poolCap;
     if (poolReserved > (long long)dPool.n) throw std::runtime_error("internal: end-location pool of the device stage too small");
     const int* dList = nullptr;

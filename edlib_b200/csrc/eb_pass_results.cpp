@@ -296,13 +296,9 @@ void Pass::collect_ends(const std::vector<int>* pairs) {
     };
     const size_t M = pairs ? pairs->size() : (size_t)N;
     auto pair_of = [&](size_t j) -> int { return pairs ? (*pairs)[j] : (int)j; };
-    const size_t nparts = host_parts(M, 65536);
-    std::vector<long long> partCount(nparts + 1, 0);
-    std::vector<int> bad(nparts, 0);
-    auto run = [&](const std::function<void(size_t, size_t, size_t)>& fn) {
-        HostPool::get().run(nparts, [&](size_t t) { fn(t, M * t / nparts, M * (t + 1) / nparts); });
-    };
-    run([&](size_t t, size_t lo, size_t hi) {
+    std::vector<long long> partCount(HostPool::get().width() + 1, 0);
+    std::vector<int> bad(HostPool::get().width(), 0);
+    const size_t nparts = parallel_parts(M, 65536, [&](size_t t, size_t lo, size_t hi) {
         long long c = 0;
         for (size_t j = lo; j < hi; ++j) {
             const int i = pair_of(j);
@@ -319,7 +315,7 @@ void Pass::collect_ends(const std::vector<int>* pairs) {
         partCount[t + 1] += partCount[t];
     }
     p->endPool.resize((size_t)partCount[nparts]);
-    run([&](size_t t, size_t lo, size_t hi) {
+    parallel_parts(M, 65536, [&](size_t t, size_t lo, size_t hi) {
         long long at = partCount[t];
         for (size_t j = lo; j < hi; ++j) {
             const int i = pair_of(j);
@@ -373,11 +369,10 @@ void Pass::res_begin() {
     if (resUploaded) return;
     resUploaded = true;
     // word classes that hold found pairs; bit 0: found pairs the lane kernel cannot take (long queries, big alphabets)
-    const size_t nparts = host_parts((size_t)N, 65536);
-    std::vector<unsigned> part(nparts, 0u);
-    HostPool::get().run(nparts, [&](size_t t) {
+    std::vector<unsigned> part(HostPool::get().width(), 0u);
+    parallel_parts((size_t)N, 65536, [&](size_t t, size_t lo, size_t hi) {
         unsigned bits = 0;
-        for (size_t i = (size_t)N * t / nparts, hi = (size_t)N * (t + 1) / nparts; i < hi; ++i) {
+        for (size_t i = lo; i < hi; ++i) {
             if (p->ed[i] < 0 || p->special[i]) continue;
             const int m = p->qlen[i];
             bits |= (m > 0 && m <= 256) ? (1u << ((m + 31) / 32)) : 1u;
@@ -485,18 +480,13 @@ void Pass::paths_device() {
         rStartPool.alloc(be, p->startPool.size());
         rStartPool.upload(p->startPool.data(), p->startPool.size());
     }
-    int maxEd = 0;
-    {
-        const size_t nparts = host_parts((size_t)N, 65536);
-        std::vector<int> part(nparts, 0);
-        HostPool::get().run(nparts, [&](size_t t) {
-            int mx = 0;
-            for (size_t i = (size_t)N * t / nparts, hi = (size_t)N * (t + 1) / nparts; i < hi; ++i) mx = std::max(mx, p->ed[i]);
-            part[t] = mx;
-        });
-        for (int v : part) maxEd = std::max(maxEd, v);
-    }
-    resMaxEd = maxEd;
+    std::vector<int> partMax(HostPool::get().width(), 0);
+    parallel_parts((size_t)N, 65536, [&](size_t t, size_t lo, size_t hi) {
+        int mx = 0;
+        for (size_t i = lo; i < hi; ++i) mx = std::max(mx, p->ed[i]);
+        partMax[t] = mx;
+    });
+    resMaxEd = *std::max_element(partMax.begin(), partMax.end());
     DevBuf<long long> dAlnStart(be, (size_t)N);
     DevBuf<int> dAlnLen(be, (size_t)N);
     be->fill(dAlnStart.p, 0xff, (size_t)N * sizeof(long long));  // -1: no path
@@ -653,15 +643,8 @@ void Pass::paths() {
         std::vector<Node> nodes;
         std::vector<int> rootOf, frontier, leaves;
         paths_device();  // every found pair of the lane kernel's word classes (or nothing)
-        {
-            std::atomic<int> open(0);  // found pairs the device did not handle (long queries, long target slices)
-            parallel_ranges((size_t)N, 65536, [&](size_t lo, size_t hi) {
-                bool any = false;
-                for (size_t i = lo; i < hi && !any; ++i) any = p->ed[i] >= 0 && p->alnStart[i] < 0;
-                if (any) open.store(1, std::memory_order_relaxed);
-            });
-            if (!open.load()) return;
-        }
+        // found pairs the device did not handle (long queries, long target slices)
+        if (!parallel_any((size_t)N, 65536, [&](size_t i) { return p->ed[i] >= 0 && p->alnStart[i] < 0; })) return;
         rootOf.assign(N, -1);
         for (int i = 0; i < N; ++i) {
             if (p->ed[i] < 0 || p->alnStart[i] >= 0) continue;  // no result / done on the device
