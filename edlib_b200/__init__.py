@@ -12,7 +12,7 @@ import re as _re
 from ._ffi import (EDLIB_CIGAR_EXTENDED, EDLIB_CIGAR_STANDARD, EDLIB_STATUS_OK, MODES, TASKS, EdlibLib,
                    product_path)
 
-__all__ = ["align", "align_batch", "align_many", "getNiceAlignment", "library"]
+__all__ = ["align", "align_batch", "align_many", "find_hits", "getNiceAlignment", "library"]
 
 _lib = None
 
@@ -111,6 +111,30 @@ def align_batch(queries, targets, mode="NW", task="distance", k=-1, additionalEq
 
 
 align_many = align_batch  # the name SURVEY.md 8f proposes for the batched binding entry
+
+
+def find_hits(queries, target, k, strands="forward", max_hits=None, additionalEqualities=None):
+    """Every place where each query occurs in `target` with at most k edits (HW mode; queries of 1..256 symbols).
+
+    Returns one dict per query: {"count": number of hits, "hits": [(column, score), ...]}, where the hits are every
+    end column c of `target` whose best alignment of the query ending there has score <= k, in ascending columns.
+    At most `max_hits` hits are listed per query (None: all); "count" is always the full number.
+    strands="both": the reverse complement is searched too; its hits follow the forward ones and every hit becomes
+    (column, score, "+" or "-").  The sequence rules are those of `align_batch`."""
+    if strands not in ("forward", "both"):
+        raise ValueError("strands must be 'forward' or 'both'")
+    queries = list(queries)
+    if strands == "both" and not all(_is_plain(s) for s in queries + [target]):
+        raise ValueError("strands='both' needs bytes or ASCII str sequences")
+    mapped, eqs = _map_to_bytes(queries + [target], additionalEqualities)
+    both = strands == "both"
+    st, res = library().find_hits(mapped[:-1], mapped[-1], k, both, (1 << 62) if max_hits is None else max_hits, eqs)
+    if st != EDLIB_STATUS_OK:
+        raise Exception("There was an error. (" + library().lib.edlibB200LastError().decode() + ")")
+    if both:
+        for r in res:
+            r["hits"] = [(c, s, "-" if d else "+") for c, s, d in r["hits"]]
+    return res
 
 
 def getNiceAlignment(alignResult, query, target, gapSymbol="-"):

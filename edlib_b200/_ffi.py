@@ -34,7 +34,13 @@ class AlignResult(C.Structure):           # include/edlib.h EdlibAlignResult (48
                 ("alignmentLength", C.c_int), ("alphabetLength", C.c_int)]
 
 
+class Hits(C.Structure):                  # include/edlib_b200.h EdlibB200Hits (48 bytes)
+    _fields_ = [("numQueries", C.c_int), ("counts", C.POINTER(C.c_longlong)), ("offsets", C.POINTER(C.c_longlong)),
+                ("columns", C.POINTER(C.c_int)), ("scores", C.POINTER(C.c_int)), ("strands", C.POINTER(C.c_ubyte))]
+
+
 assert C.sizeof(EqualityPair) == 2 and C.sizeof(AlignConfig) == 32 and C.sizeof(AlignResult) == 48
+assert C.sizeof(Hits) == 48
 
 
 def make_config(k=-1, mode=EDLIB_MODE_NW, task=EDLIB_TASK_DISTANCE, equalities=None):
@@ -136,6 +142,34 @@ class EdlibLib:
         strands = (C.c_ubyte * max(len(queries), 1))()
         st, out = self._run_batch(lambda *a: fn(*a, strands), queries, targets, k, mode, task, equalities)
         return st, out, [strands[i] for i in range(len(queries))]
+
+    def find_hits(self, queries, target, k, both=False, max_hits=(1 << 62), equalities=None,
+                  mode=EDLIB_MODE_HW, task=EDLIB_TASK_DISTANCE):
+        """edlibB200FindHits over one shared target.  Returns (status, [{"count": int, "hits": [...]}]) with hits
+        (column, score), or (column, score, strand) when both strands were searched; status != 0: (status, None)."""
+        fn = self.lib.edlibB200FindHits
+        fn.restype = C.c_int
+        fn.argtypes = [C.POINTER(C.c_char_p), C.POINTER(C.c_int), C.c_int, C.c_char_p, C.c_int, AlignConfig, C.c_int,
+                       C.c_longlong, C.POINTER(Hits)]
+        self.lib.edlibB200FreeHits.restype = None
+        self.lib.edlibB200FreeHits.argtypes = [C.POINTER(Hits)]
+        n = len(queries)
+        cfg, keep = make_config(k, mode, task, equalities)
+        qptr = (C.c_char_p * max(n, 1))(*queries)
+        qlen = (C.c_int * max(n, 1))(*[len(q) for q in queries])
+        h = Hits()
+        st = fn(qptr, qlen, n, target, len(target), cfg, 1 if both else 0, max_hits, C.byref(h))
+        del keep
+        if st != EDLIB_STATUS_OK:
+            return st, None
+        out = []
+        for i in range(n):
+            a, b = h.offsets[i], h.offsets[i + 1]
+            cols, scores = h.columns[a:b], h.scores[a:b]
+            hits = list(zip(cols, scores, h.strands[a:b])) if both else list(zip(cols, scores))
+            out.append({"count": h.counts[i], "hits": hits})
+        self.lib.edlibB200FreeHits(C.byref(h))
+        return st, out
 
     def _run_batch(self, call, queries, targets, k, mode, task, equalities):
         n = len(queries)

@@ -24,6 +24,7 @@ namespace eb {
 void host_parallel_ranges(size_t n, size_t grain, const std::function<void(size_t, size_t)>& fn);  // eb_engine.cpp
 void free_result_arrays(EdlibAlignResult* results, size_t lo, size_t hi);  // eb_engine.cpp: frees and clears them
 void fail_results(EdlibAlignResult* results, int n);  // eb_engine.cpp: error results (status, distance -1, no arrays)
+void free_hits(EdlibB200Hits* h);  // eb_engine.cpp: frees the arrays of a hit list and clears it
 Backend* create_backend(std::string* err);  // provided by the backend object linked into this library
 int select_device(int device, std::string* err);  // 0 on success
 }
@@ -459,6 +460,57 @@ EDLIB_API void edlibB200FreeCigars(char** cigars, int n) {
     }
     std::lock_guard<std::mutex> lock(g_mu);  // the host pool serves one client at a time
     eb::host_parallel_ranges((size_t)n, 16384, free_range);
+}
+
+// What edlibB200FindHits refuses (include/edlib_b200.h), or nullptr.
+static const char* hits_input_error(const char* const* queries, const int* queryLengths, int numQueries, const char* target,
+                                    int targetLength, const EdlibAlignConfig& config, int bothStrands, long long maxHits) {
+    if (numQueries < 0) return "edlibB200FindHits: numQueries < 0";
+    if (numQueries > 0 && (!queries || !queryLengths)) return "edlibB200FindHits: no queries";
+    if (bothStrands && numQueries > 0x3fffffff) return "edlibB200FindHits: too many queries for both strands";
+    if (!target || targetLength < 1) return "edlibB200FindHits: the target must have at least one symbol";
+    if (config.mode != EDLIB_MODE_HW) return "edlibB200FindHits: mode must be EDLIB_MODE_HW";
+    if (config.task != EDLIB_TASK_DISTANCE) return "edlibB200FindHits: task must be EDLIB_TASK_DISTANCE";
+    if (config.k < 0) return "edlibB200FindHits: k must be >= 0";
+    if (maxHits < 0) return "edlibB200FindHits: maxHitsPerQuery must be >= 0";
+    if (config.additionalEqualitiesLength > 0 && !config.additionalEqualities) return "edlibB200FindHits: no equality pairs";
+    for (int i = 0; i < numQueries; ++i)
+        if (!queries[i] || queryLengths[i] < 1 || queryLengths[i] > 256) return "edlibB200FindHits: query lengths must be 1 .. 256";
+    return nullptr;
+}
+
+EDLIB_API int edlibB200FindHits(const char* const* queries, const int* queryLengths, int numQueries, const char* target,
+                                int targetLength, const EdlibAlignConfig config, int bothStrands, long long maxHitsPerQuery,
+                                EdlibB200Hits* hits) {
+    std::lock_guard<std::mutex> lock(g_mu);
+    eb::Engine* e = engine_locked();
+    if (hits) memset(hits, 0, sizeof(*hits));
+    if (!e) return EDLIB_STATUS_ERROR;  // no usable device: there is no CPU path
+    t_lastEngine = e;
+    const char* bad = hits ? hits_input_error(queries, queryLengths, numQueries, target, targetLength, config, bothStrands,
+                                              maxHitsPerQuery)
+                           : "edlibB200FindHits: hits is NULL";
+    if (bad) {
+        e->lastError = bad;
+        return EDLIB_STATUS_ERROR;
+    }
+    if (numQueries == 0) {
+        hits->offsets = static_cast<long long*>(calloc(1, sizeof(long long)));
+        hits->counts = static_cast<long long*>(malloc(sizeof(long long)));
+        if (hits->offsets && hits->counts) return EDLIB_STATUS_OK;
+        eb::free_hits(hits);
+        e->lastError = "out of memory for the hit lists";
+        return EDLIB_STATUS_ERROR;
+    }
+    const std::vector<const char*> targets((size_t)numQueries, target);
+    const std::vector<int> targetLengths((size_t)numQueries, targetLength);
+    eb::BatchInput in{queries, queryLengths, targets.data(), targetLengths.data(), numQueries, config};
+    in.strands = bothStrands != 0;
+    return e->find_hits(in, maxHitsPerQuery, hits);
+}
+
+EDLIB_API void edlibB200FreeHits(EdlibB200Hits* hits) {
+    if (hits) eb::free_hits(hits);
 }
 
 EDLIB_API void edlibB200LastStats(EdlibB200Stats* s) {

@@ -379,6 +379,35 @@ struct FinParams {
 };
 
 // ---------------------------------------------------------------------------------------------
+// Hits: every end column c of a read whose last-row score D(c) is <= k (edlibB200FindHits).  The jobs are the seed
+// windows of a K1W launch (kInit = k + 1, as planned) or the (chunk, read) items of a K1 launch over the whole target
+// (kInit = k; a chunk reports the columns it owns).  Each launch runs twice over the same jobs: the count pass writes
+// the hits of every job, the fill pass re-sweeps the jobs with room > 0 and stores their first `room` hits in column
+// order at at[job].
+// ---------------------------------------------------------------------------------------------
+struct HitParams {
+    int* count;              // count pass (at == nullptr): [job] hits of the job
+    const long long* at;     // fill pass: [job] first slot of the job's stored hits in cols / scores
+    const int* room;         // fill pass: [job] hits of the job that are stored (0: the job is skipped)
+    int* cols;               // fill pass: end columns
+    int* scores;             // fill pass: D(column)
+};
+// Per read of a hits launch: the jobs of read `slot` are plan[slot].first .. + count (windows, in column order), or
+// slot + c * numReads for c < chunks (chunks, in column order).
+struct HitPlaceParams {
+    const SeedPlan* plan;    // windows, or nullptr: chunks
+    int chunks;
+    int numReads;
+    const int* readList;     // [numReads] pair of each slot
+    const int* count;        // [job] hits of the job (count pass)
+    long long* pairCount;    // hits_total: [pair] hits of the read (reads without windows: 0)
+    const long long* pairBase;   // hits_place: [pair] first slot of the read's stored hits
+    const long long* pairStored; // hits_place: [pair] hits of the read that are stored
+    long long* at;           // hits_place: [job] -> HitParams::at
+    int* room;               // hits_place: [job] -> HitParams::room
+};
+
+// ---------------------------------------------------------------------------------------------
 // Start locations and alignment paths of short queries (<= 256 rows) WITHOUT the host in the loop: the jobs of the
 // lane kernel (reversed SHW sweeps of ref cpp:253-257; matrix-storing NW sweeps + traceback of ref cpp:276-289,
 // 1161-1213) are derived on the device from the per-pair results, and their outcome is written straight into the

@@ -10,6 +10,8 @@
 //   myersCalcEditDistanceSemiGlobal 550-704, myersCalcEditDistanceNW 730-928 -> k1_* / w_sweep
 //   obtainAlignmentTraceback 942-1141 -> traceback_job
 #pragma once
+#include <type_traits>
+
 #include "eb_common.h"
 
 #if defined(__CUDA_ARCH__)
@@ -361,6 +363,37 @@ EB_HD void k1_event(K1State<NW>& st, int score, int column, RecT* rec, int recId
     st.cnt++;
 }
 
+// Hits of one job of a hits launch (eb_common.h: HitParams), in the order the sweep meets them (ascending columns):
+// all are counted, the first `room` stored.  Sweeps that record into a HitSink compare against a fixed threshold
+// (st.best / K1Band::best stays k) instead of a running minimum.
+struct HitSink {
+    int count, room;
+    int* cols;
+    int* scores;
+    EB_HD void hit(int score, int column) {
+        if (count < room) {
+            cols[count] = column;
+            scores[count] = score;
+        }
+        ++count;
+    }
+};
+// The sink of job `job`, or false in a fill pass when nothing of the job is stored.
+EB_HD bool hit_sink_open(const HitParams& h, int job, HitSink& s) {
+    s.count = 0;
+    s.room = h.at ? h.room[job] : 0;
+    s.cols = h.at ? h.cols + h.at[job] : nullptr;
+    s.scores = h.at ? h.scores + h.at[job] : nullptr;
+    return !h.at || s.room > 0;
+}
+EB_HD void hit_sink_close(const HitParams& h, int job, const HitSink& s) {
+    if (!h.at) h.count[job] = s.count;
+}
+template <int NW, bool RANGE = false>
+EB_HD void k1_event(K1State<NW>&, int score, int column, HitSink* sink, int, Ovf*, int*, int) {
+    sink->hit(score, column);
+}
+
 // Target symbols addressed through a plain pointer (host emulation; any directly addressable
 // target).  The device kernel substitutes a reader over its shared-memory tile.
 struct PtrSyms {
@@ -612,12 +645,14 @@ struct K1Band {
         VP1 = HN1 | ~(X1 | HP1);
         S += 1 - (int)(HN1 >> 31);
         if (TRACK && j >= lo) {
-            constexpr int CAP = (int)(sizeof(rec->pos) / sizeof(rec->pos[0]));
             const int kb = kb0 - j;  // 0..63
             const uint64_t M = kb >= 63 ? 0ull : (~0ull << (kb + 1));
             const int score = S - popcount32(VP0 & (uint32_t)M) - popcount32(VP1 & (uint32_t)(M >> 32)) +
                               popcount32(VN0 & (uint32_t)M) + popcount32(VN1 & (uint32_t)(M >> 32));
-            if (score <= best) {  // same bookkeeping as k1_event (ref cpp:658-673)
+            if constexpr (std::is_same<RecT, HitSink>::value) {
+                if (score <= best) rec->hit(score, ws + j);  // hits: best is the fixed threshold
+            } else if (score <= best) {  // same bookkeeping as k1_event (ref cpp:658-673)
+                constexpr int CAP = (int)(sizeof(rec->pos) / sizeof(rec->pos[0]));
                 if (score < best) {
                     best = score;
                     cnt = 0;
@@ -690,11 +725,9 @@ EB_HD void k1b_sweep(const WAcc& acc, const uint8_t* tsyms, int ws, int m, int o
 // L2-resident).  The profile rows have NW + 4 words: two words of ones (wildcard rows above the query, used by
 // the banded sweep), the NW-word K1 profile, two words of zeros.  Windows whose end columns of interest span at
 // most 64 diagonals take the banded sweep (k1b_sweep: 2 words per column instead of NW), the others the full one.
+// The profile rows of a K1W work item (the layout above), shared by k1w_thread and k1w_hits_thread.
 template <int NW, class WAcc>
-EB_HD void k1w_thread(const K1WParams& p, int slot, WAcc& acc) {
-    const int pair = p.readList[slot];
-    const int m = p.qlen[pair];
-    WinRec* rec = p.recs + slot;
+EB_HD void k1w_profile(const K1WParams& p, int pair, int m, WAcc& acc) {
     for (int code = 0; code < p.ncodes; ++code) {
         acc.store_word(code, 0, ~0u);
         acc.store_word(code, 1, ~0u);
@@ -703,6 +736,14 @@ EB_HD void k1w_thread(const K1WParams& p, int slot, WAcc& acc) {
     }
     K1View<NW, WAcc> k1acc{acc};
     k1_build_peq<NW>(k1acc, p.qcodes + p.qoff[pair], m, MODE_HW, p.ncodes, p.eqtab);
+}
+template <int NW, class WAcc>
+EB_HD void k1w_thread(const K1WParams& p, int slot, WAcc& acc) {
+    const int pair = p.readList[slot];
+    const int m = p.qlen[pair];
+    WinRec* rec = p.recs + slot;
+    k1w_profile<NW>(p, pair, m, acc);
+    K1View<NW, WAcc> k1acc{acc};
     const int ws = p.winStart[slot], tf = p.trackFrom[slot], len = p.winLen[slot];
     const int kInit = p.kInit[slot];
     const int t = kInit - 1;
@@ -735,6 +776,89 @@ EB_HD void k1w_thread(const K1WParams& p, int slot, WAcc& acc) {
         k1_columns<NW, false, true>(st, k1acc, PtrSyms{p.tcodes + ws + tf}, len - tf, ws + tf, rec, slot, p.ovf, p.ovfCount, p.ovfCap);
     rec->best = st.best;
     rec->cnt = st.cnt;
+}
+
+// Hits of one window job (eb_common.h: HitParams): the sweeps of k1w_thread with the window's threshold t = kInit - 1
+// held fixed; every tracked column scoring <= t is a hit.  The tracked columns of a read's windows cover every end
+// column of every alignment within t, and every such score is exact (seed_windows), so the hits of a read are those of
+// its windows in window order.  The early exits stay valid: they only leave windows that hold no score <= t.
+template <int NW, class WAcc>
+EB_HD void k1w_hits_thread(const K1WParams& p, const HitParams& h, int slot, WAcc& acc) {
+    HitSink sink;
+    if (!hit_sink_open(h, slot, sink)) return;
+    const int pair = p.readList[slot];
+    const int m = p.qlen[pair];
+    k1w_profile<NW>(p, pair, m, acc);
+    K1View<NW, WAcc> k1acc{acc};
+    const int ws = p.winStart[slot], tf = p.trackFrom[slot], len = p.winLen[slot];
+    const int t = p.kInit[slot] - 1;
+    const int hi = len - 1;
+    if (t >= 0 && (hi - tf) + 2 * t + 1 <= 64) {
+        const int c0 = tf - (m + t) > 0 ? tf - (m + t) : 0;
+        int best = t, cnt = 0;
+        k1b_sweep(acc, p.tcodes + ws, ws, m, 32 * NW - m, c0, tf, hi, t, p.checkAfter, best, cnt, &sink, p, slot);
+    } else {
+        K1State<NW> st;
+        k1_init<NW>(st, m, t);
+        bool hopeless = false;
+        for (int j = 0; j < tf; j += 32) {
+            const int cntj = tf - j < 32 ? tf - j : 32;
+            k1_columns<NW, false, false>(st, k1acc, PtrSyms{p.tcodes + ws + j}, cntj, ws + j, &sink, slot, nullptr, nullptr, 0);
+            if (st.up - st.down - (len - (j + cntj)) > t) {
+                hopeless = true;
+                break;
+            }
+        }
+        if (!hopeless)
+            k1_columns<NW, false, true>(st, k1acc, PtrSyms{p.tcodes + ws + tf}, len - tf, ws + tf, &sink, slot, nullptr, nullptr, 0);
+    }
+    hit_sink_close(h, slot, sink);
+}
+
+// Hits of one (chunk, read) job of a whole-target HW sweep (K1Params chunk geometry, kInit = k): the chunk restarts
+// halo >= 2m columns early, so every score of the columns it owns is exact, and it reports only those.
+template <int NW, class Acc>
+EB_HD void k1_hits_thread(const K1Params& p, const HitParams& h, int slot, int chunk, Acc& acc) {
+    const int job = chunk * p.numReads + slot;
+    HitSink sink;
+    if (!hit_sink_open(h, job, sink)) return;
+    const int pair = p.readList[slot];
+    const int m = p.qlen[pair];
+    k1_build_peq<NW>(acc, p.qcodes + p.qoff[pair], m, MODE_HW, p.ncodes, p.eqtab);
+    K1State<NW> st;
+    k1_init<NW>(st, m, p.kInit[slot]);
+    const K1Chunk g = k1_chunk(p, chunk);
+    k1_columns<NW, false, false>(st, acc, PtrSyms{p.tcodes + g.hs}, g.cs - g.hs, g.hs, &sink, job, nullptr, nullptr, 0);
+    k1_columns<NW, false, true>(st, acc, PtrSyms{p.tcodes + g.cs}, g.ce - g.cs, g.cs, &sink, job, nullptr, nullptr, 0);
+    hit_sink_close(h, job, sink);
+}
+
+// Job j of read `slot` of a hits launch (eb_common.h: HitPlaceParams), j = 0 .. hit_jobs(p, slot) - 1, in column order.
+EB_HD int hit_jobs(const HitPlaceParams& p, int slot) {
+    if (!p.plan) return p.chunks;
+    return p.plan[slot].state == SEED_WINDOWS ? p.plan[slot].count : 0;
+}
+EB_HD int hit_job(const HitPlaceParams& p, int slot, int j) { return p.plan ? p.plan[slot].first + j : slot + j * p.numReads; }
+// After the count pass: the hits of the read.
+EB_HD void hits_total_item(const HitPlaceParams& p, int slot) {
+    long long total = 0;
+    for (int j = 0, n = hit_jobs(p, slot); j < n; ++j) total += p.count[hit_job(p, slot, j)];
+    p.pairCount[p.readList[slot]] = total;
+}
+// Before the fill pass: where each job of the read stores its hits, and how many of them (the read's first
+// pairStored hits in column order).
+EB_HD void hits_place_item(const HitPlaceParams& p, int slot) {
+    const int pair = p.readList[slot];
+    const long long base = p.pairBase[pair], stored = p.pairStored[pair];
+    long long done = 0;
+    for (int j = 0, n = hit_jobs(p, slot); j < n; ++j) {
+        const int job = hit_job(p, slot, j);
+        const int c = p.count[job];
+        const long long left = stored - done;
+        p.at[job] = base + done;
+        p.room[job] = left <= 0 ? 0 : (left < c ? (int)left : c);
+        done += c;
+    }
 }
 
 // =============================================================================================

@@ -908,6 +908,44 @@ int Engine::align_batch(const BatchInput& in, EdlibAlignResult* results, unsigne
     }
 }
 
+void free_hits(EdlibB200Hits* h) {
+    free(h->counts);
+    free(h->offsets);
+    free(h->columns);
+    free(h->scores);
+    free(h->strands);
+    memset(h, 0, sizeof(*h));
+}
+
+// The grouped batch of every query against the one target (a strand batch for both strands), then the hits pass
+// instead of the distance pass.
+int Engine::find_hits(const BatchInput& in, long long maxHits, EdlibB200Hits* out) {
+    Prepared* p = nullptr;
+    stats = EngineStats();
+    statsPending_ = false;
+    memset(out, 0, sizeof(*out));
+    try {
+        p = prepare(in);
+        be_->reset_timing();
+        {
+            Pass ps(*this, be_, p);
+            ps.hits(maxHits, out);
+        }
+        be_->sync_all();
+        be_->release_marks();
+        stats.launches = be_->launches();
+        statsPending_ = true;
+        release(p);
+        return EDLIB_STATUS_OK;
+    } catch (const std::exception& e) {
+        lastError = e.what();
+        quiesce();
+        if (p) release(p);
+        free_hits(out);
+        return EDLIB_STATUS_ERROR;
+    }
+}
+
 // =============================================================================================
 // Streamed one-shot path of edlibAlignBatch: many short reads, HW, ONE shared target, plain equality.
 //

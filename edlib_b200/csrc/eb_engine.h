@@ -8,11 +8,13 @@
 #include <stdint.h>
 
 #include <map>
+#include <stdexcept>
 #include <string>
 #include <utility>
 #include <vector>
 
 #include "../../include/edlib.h"
+#include "../../include/edlib_b200.h"
 #include "eb_common.h"
 
 namespace eb {
@@ -83,6 +85,15 @@ struct Backend {
     virtual void launch_fin_count(const FinParams& p) = 0;
     virtual void launch_fin_fill(const FinParams& p) = 0;
     virtual void launch_qalpha(const QAlphaParams& p) = 0;
+    // hits (eb_common.h: HitParams): count or fill pass over window jobs / (chunk, read) jobs of a whole-target sweep,
+    // and the per-read totals / placement between the two passes.  A backend without these kernels refuses the call.
+    virtual void launch_k1w_hits(const K1WParams&, const HitParams&, int /*nw32*/) { no_kernel("k1w_hits"); }
+    virtual void launch_k1_hits(const K1Params&, const HitParams&, int /*nw32*/) { no_kernel("k1_hits"); }
+    virtual void launch_hits_total(const HitPlaceParams&) { no_kernel("hits_total"); }
+    virtual void launch_hits_place(const HitPlaceParams&) { no_kernel("hits_place"); }
+    [[noreturn]] static void no_kernel(const char* name) {
+        throw std::runtime_error(std::string(name) + ": no such kernel on this backend");
+    }
     // timing of the launches issued since the last reset (device time, ms) and their count
     virtual void reset_timing() = 0;
     virtual double kernel_ms(const char* nameOrNull) = 0;
@@ -183,6 +194,10 @@ public:
     // One-shot streamed path for large HW batches of short reads over one shared target (eb_engine.cpp): returns
     // false when the batch is not of that shape (nothing done), throws on failure.
     bool align_streamed(const BatchInput& in, EdlibAlignResult* results);
+    // edlibB200FindHits: every end column within config.k of every query over the one shared target (in.strands: of its
+    // reverse complement too), at most maxHits stored per query.  `out` is filled with malloc'd arrays; on failure
+    // nothing stays allocated.  Returns EDLIB_STATUS_OK / EDLIB_STATUS_ERROR.
+    int find_hits(const BatchInput& in, long long maxHits, EdlibB200Hits* out);
 
     void finish_stats();  // fills the device-time fields of `stats` for the last pass (on demand)
 

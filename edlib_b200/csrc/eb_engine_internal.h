@@ -18,6 +18,7 @@
 #include <mutex>
 #include <chrono>
 #include <map>
+#include <memory>
 #include <stdexcept>
 #include <thread>
 #include <unordered_map>
@@ -716,6 +717,15 @@ struct Pass {
     void dev_finish_slice(int si);
     // After the last slice: the reads the device could not decide, grouped and run through the host-driven stages.
     void dev_leftovers();
+
+    // ---- hits (edlibB200FindHits; eb_pass_lane.cpp) ----------------------------------------------------------
+    // Runs instead of the distance pass: every end column scoring <= k of every pair over the batch's one target, into
+    // `out` (malloc'd arrays; the two pairs of a read of a strand batch share its cap, forward first).  A pair takes the
+    // seed windows of the first level whose threshold reaches k, or the whole-target sweep (no such level, saturated
+    // plan, repeats, short target, equality table); both count, place, then fill.
+    void hits(long long maxHits, EdlibB200Hits* out);
+    // The K1W launch over the first numJobs jobs (or as many as *jobs.count says, numJobs < 0), records not set.
+    K1WParams window_params(const Target& tg, const WinJobs& jobs, int numJobs) const;
 
     // Distance pass of everything else: one alignment per warp (or per thread with its own target).
     void warp_distance();

@@ -326,6 +326,40 @@ __global__ void __launch_bounds__(THREADS) k1w_kernel(const K1WParams p) {
     k1w_thread<NW>(p, slot, acc);
 }
 
+// Hits of window jobs (eb_core.h: k1w_hits_thread): the k1w_kernel shape, one count or fill pass per launch.
+template <int NW, int THREADS>
+__global__ void __launch_bounds__(THREADS) k1w_hits_kernel(const K1WParams p, const HitParams h) {
+    extern __shared__ __align__(128) unsigned char smem[];
+    const int slot = blockIdx.x * THREADS + threadIdx.x;
+    if (slot >= p.numReads) return;
+    SmemWordAcc<THREADS, NW + 4> acc;
+    acc.base = smem_u32(smem) + 4u * threadIdx.x;
+    k1w_hits_thread<NW>(p, h, slot, acc);
+}
+
+// Hits of a whole-target sweep (eb_core.h: k1_hits_thread): one thread per (read, chunk), symbols from global memory
+// (L2), the profile in shared memory as for lane_kernel.
+template <int NW>
+__global__ void k1_hits_kernel(const K1Params p, const HitParams h) {
+    extern __shared__ __align__(128) unsigned char smem[];
+    const int slot = blockIdx.x * blockDim.x + threadIdx.x;
+    if (slot >= p.numReads) return;
+    SmemPeqAcc<NW> acc;
+    acc.codeStride = (uint32_t)blockDim.x * (16u + 4u * SmemPeqAcc<NW>::NWB);
+    acc.a0 = smem_u32(smem) + 16u * threadIdx.x;
+    acc.b0 = smem_u32(smem) + 16u * blockDim.x + 4u * SmemPeqAcc<NW>::NWB * threadIdx.x;
+    k1_hits_thread<NW>(p, h, slot, (int)blockIdx.y, acc);
+}
+
+__global__ void hits_total_kernel(const HitPlaceParams p) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < p.numReads) hits_total_item(p, i);
+}
+__global__ void hits_place_kernel(const HitPlaceParams p) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < p.numReads) hits_place_item(p, i);
+}
+
 // L: one alignment per thread over its own target (eb_core.h: lane_job).
 template <int NW, int MODE, bool REV, bool STORE>
 __global__ void lane_kernel(const LParams p) {
@@ -937,6 +971,36 @@ struct CudaBackend : Backend {
                 launch("k1w", k1w_kernel<decltype(w)::value, THREADS>, (p.numReads + THREADS - 1) / THREADS, THREADS, smem, p);
             });
         });
+    }
+    void launch_k1w_hits(const K1WParams& p, const HitParams& h, int nw) override {
+        if (p.numReads <= 0) return;
+        int block = 128;
+        const size_t perThread = (size_t)p.ncodes * 4 * (nw + 4);
+        while (block > 32 && perThread * block > 96 * 1024) block >>= 1;
+        const size_t smem = perThread * block;
+        if (smem > (size_t)maxSmemOptin) throw std::runtime_error("K1W: alphabet too large for shared memory");
+        with_nw(nw, [&](auto w) {
+            with_one_of<128, 64, 32>(block, "bad K1W CTA size", [&](auto threads) {
+                constexpr int THREADS = decltype(threads)::value;
+                launch("k1w_hits", k1w_hits_kernel<decltype(w)::value, THREADS>, (p.numReads + THREADS - 1) / THREADS, THREADS, smem, p, h);
+            });
+        });
+    }
+    void launch_k1_hits(const K1Params& p, const HitParams& h, int nw) override {
+        if (p.numReads <= 0 || p.chunks <= 0) return;
+        int block = 128;
+        const size_t perThread = (size_t)p.ncodes * (16 + 4 * (nw > 4 ? nw - 4 : 0));
+        while (block > 32 && perThread * block > 96 * 1024) block >>= 1;
+        const size_t smem = perThread * block;
+        if (smem > (size_t)maxSmemOptin) throw std::runtime_error("K1: alphabet too large for shared memory");
+        const dim3 grid((p.numReads + block - 1) / block, p.chunks);
+        with_nw(nw, [&](auto w) { launch("k1_hits", k1_hits_kernel<decltype(w)::value>, grid, block, smem, p, h); });
+    }
+    void launch_hits_total(const HitPlaceParams& p) override {
+        if (p.numReads > 0) launch("hits_total", hits_total_kernel, (p.numReads + 255) / 256, 256, 0, p);
+    }
+    void launch_hits_place(const HitPlaceParams& p) override {
+        if (p.numReads > 0) launch("hits_place", hits_place_kernel, (p.numReads + 255) / 256, 256, 0, p);
     }
     void launch_lane(const LParams& p, int nw, int mode, bool rev, bool store) override {
         int block = 128;

@@ -119,7 +119,7 @@ int Pass::plan_windows(SeedPlanParams sp, WinJobs& jobs, int cap, bool hostCount
     }
 }
 
-void Pass::sweep_windows(const Target& tg, int nw, const WinJobs& jobs, int numJobs, const WinRecords& out) {
+K1WParams Pass::window_params(const Target& tg, const WinJobs& jobs, int numJobs) const {
     K1WParams wp;
     memset(&wp, 0, sizeof(wp));
     wp.tcodes = p->dSeq.p + tg.off;
@@ -136,6 +136,11 @@ void Pass::sweep_windows(const Target& tg, int nw, const WinJobs& jobs, int numJ
     wp.checkAfter = tun.windowCheckAfter;
     wp.ncodes = p->ncodes;
     wp.eqtab = p->hasEq ? p->dEqtab.p : nullptr;
+    return wp;
+}
+
+void Pass::sweep_windows(const Target& tg, int nw, const WinJobs& jobs, int numJobs, const WinRecords& out) {
+    K1WParams wp = window_params(tg, jobs, numJobs);
     wp.recs = out.recs;
     wp.ovf = out.ovf;
     wp.ovfCount = out.ovfCount;
@@ -927,5 +932,225 @@ void Pass::dev_leftovers() {
     }
     trace.mark("device stage: leftovers grouped");
     for (auto& kv : groups) lane_group(kv.first.first, kv.first.second, kv.second.pairs, &kv.second.excl, &kv.second.bound, 1);
+}
+// =============================================================================================
+// Hits (edlibB200FindHits): every end column within k instead of the minimum.  The seed levels are exact pigeonhole
+// filters: planned with threshold k, the tracked columns of a read's windows cover every end column of every alignment
+// within k, hold every such score exactly and are disjoint and in column order; the whole-target sweep restarts each
+// chunk 2m columns early and reports the columns the chunk owns.  Either way a read's hits are those of its jobs in
+// job order, so no sort is needed: count per job, total per read, the read's place in the output (host), the place of
+// each job, and a fill pass over the jobs that store something.
+// =============================================================================================
+namespace {
+// One launch group of the hits pass: reads of one word class on one route, with what the fill pass needs again.
+struct HitRun {
+    int nw = 0, level = -1;  // seed level, or -1: whole-target sweep
+    std::vector<int> pairs;
+    DevBuf<int> dList, dCount, dRoom, dWinCount;
+    DevBuf<long long> dAt;
+    DevBuf<SeedPlan> dPlan;  // seed route
+    WinJobs jobs;            // seed route
+    DevBuf<int> dK;          // whole-target sweep: k per read
+    int numJobs = 0, chunks = 0, chunkLen = 0;
+};
+constexpr int HIT_RUN_READS = 1 << 18;  // reads per launch group (bounds the per-job arrays of a whole-target sweep)
+}  // namespace
+
+void Pass::hits(long long maxHits, EdlibB200Hits* out) {
+    if (p->tg.size() != 1) throw std::runtime_error("internal: hits need one shared target");
+    const Target& tg = p->tg[0];
+    const int n = tg.len;
+    const int Q = p->strands ? N / 2 : N;
+    // ---- routes: the first seed level whose threshold reaches k itself, else the whole-target sweep ----
+    const bool seeds = n >= tun.filterMinTarget && !p->hasEq && tun.filterSeedK > 0 && tun.filterSeedLevels > 0 && seed_index(0);
+    std::vector<std::unique_ptr<HitRun>> runs;
+    std::vector<int> full[9];
+    {
+        std::map<std::pair<int, int>, std::vector<int>> groups;  // (level, nw) -> pairs
+        for (int pair = 0; pair < N; ++pair) {
+            const int m = p->qlen[pair], nw = ceil_div(m, 32);
+            int level = -1;
+            for (int l = 0; seeds && l < tun.filterSeedLevels && level < 0; ++l)
+                if (seedIdx->Ls[l] > 0 && seed_threshold(m, k, seedIdx->Ls[l], tun.filterSeedK, -1) == k) level = l;
+            if (level < 0) full[nw].push_back(pair);
+            else groups[std::make_pair(level, nw)].push_back(pair);
+        }
+        for (auto& kv : groups)
+            for (size_t a = 0; a < kv.second.size(); a += HIT_RUN_READS) {
+                runs.emplace_back(new HitRun());
+                HitRun& r = *runs.back();
+                r.level = kv.first.first;
+                r.nw = kv.first.second;
+                r.pairs.assign(kv.second.begin() + a, kv.second.begin() + std::min(kv.second.size(), a + HIT_RUN_READS));
+            }
+    }
+    DevBuf<long long> dPairCount(be, (size_t)N);
+    be->zero(dPairCount.p, (size_t)N * sizeof(long long));
+    // ---- count pass of the seed route: plan at threshold k (one host wait for the window count, one for the plans) ----
+    for (auto& rp : runs) {
+        HitRun& r = *rp;
+        const int g = (int)r.pairs.size();
+        r.dList.alloc(be, g);
+        r.dList.upload(r.pairs.data(), g);
+        const std::vector<int> thr((size_t)g, k);
+        DevBuf<int> dThr(be, g);
+        dThr.upload(thr.data(), g);
+        r.dPlan.alloc(be, g);
+        r.dWinCount.alloc(be, 1);
+        be->zero(r.dWinCount.p, sizeof(int));
+        SeedPlanParams sp = seed_plan_params(tg, r.level);
+        sp.readList = r.dList.p;
+        sp.thr = dThr.p;
+        sp.numReads = g;
+        sp.maxLen = 32 * r.nw;
+        sp.plan = r.dPlan.p;
+        r.jobs.count = r.dWinCount.p;
+        const int perRead = r.level == 0 ? 8 : r.level == 1 ? 96 : r.level == 2 ? 400 : 1500;
+        r.numJobs = plan_windows(sp, r.jobs, (int)std::min<long long>((long long)g * perRead + 4096, 1LL << 28), true);
+        std::vector<SeedPlan> plan((size_t)g);
+        be->d2h(plan.data(), r.dPlan.p, (size_t)g * sizeof(SeedPlan));
+        stats.d2hBytes += (long long)g * (long long)sizeof(SeedPlan);
+        stats.filterWindows += r.numJobs;
+        for (int s = 0; s < g; ++s) {
+            // saturated: more candidates than the level holds, seeds of repeats, or no room in the job arrays
+            if (plan[(size_t)s].state == SEED_SATURATED) full[r.nw].push_back(r.pairs[(size_t)s]);
+            else stats.filterDecided++;
+        }
+        r.dCount.alloc(be, (size_t)std::max(r.numJobs, 1));
+        if (r.numJobs > 0) {
+            const HitParams h{r.dCount.p, nullptr, nullptr, nullptr, nullptr};
+            be->launch_k1w_hits(window_params(tg, r.jobs, r.numJobs), h, r.nw);
+        }
+        HitPlaceParams hp;
+        memset(&hp, 0, sizeof(hp));
+        hp.plan = r.dPlan.p;
+        hp.numReads = g;
+        hp.readList = r.dList.p;
+        hp.count = r.dCount.p;
+        hp.pairCount = dPairCount.p;
+        be->launch_hits_total(hp);
+    }
+    trace.mark("hits: seed windows counted");
+    // ---- count pass of the whole-target sweep (launched after the seed route: it overwrites the totals of saturated reads) ----
+    K1Params kp;
+    memset(&kp, 0, sizeof(kp));
+    kp.tcodes = p->dSeq.p + tg.off;
+    kp.n = n;
+    kp.qcodes = p->dSeq.p;
+    kp.qoff = p->dQoff.p;
+    kp.qlen = p->dQlen.p;
+    kp.mode = MODE_HW;
+    kp.ncodes = p->ncodes;
+    kp.eqtab = p->hasEq ? p->dEqtab.p : nullptr;
+    const size_t seedRuns = runs.size();
+    for (int nw = 1; nw <= 8; ++nw)
+        for (size_t a = 0; a < full[nw].size(); a += HIT_RUN_READS) {
+            runs.emplace_back(new HitRun());
+            HitRun& r = *runs.back();
+            r.nw = nw;
+            r.pairs.assign(full[nw].begin() + a, full[nw].begin() + std::min(full[nw].size(), a + HIT_RUN_READS));
+            const int g = (int)r.pairs.size();
+            stats.filterFallback += g;
+            const LaneGroup c{0, nw, r.pairs, tg, n, {}, {}, {}, {}};
+            lane_geometry(c, g, nw, r.chunks, r.chunkLen, true);
+            r.numJobs = r.chunks * g;
+            r.dList.alloc(be, g);
+            r.dList.upload(r.pairs.data(), g);
+            const std::vector<int> kk((size_t)g, k);
+            r.dK.alloc(be, g);
+            r.dK.upload(kk.data(), g);
+            r.dCount.alloc(be, (size_t)r.numJobs);
+            kp.readList = r.dList.p;
+            kp.kInit = r.dK.p;
+            kp.numReads = g;
+            kp.chunks = r.chunks;
+            kp.chunkLen = r.chunkLen;
+            kp.halo = 64 * nw;
+            const HitParams h{r.dCount.p, nullptr, nullptr, nullptr, nullptr};
+            be->launch_k1_hits(kp, h, nw);
+            stats.k1Cells += (long long)g * 32 * nw * (long long)n;
+            HitPlaceParams hp;
+            memset(&hp, 0, sizeof(hp));
+            hp.chunks = r.chunks;
+            hp.numReads = g;
+            hp.readList = r.dList.p;
+            hp.count = r.dCount.p;
+            hp.pairCount = dPairCount.p;
+            be->launch_hits_total(hp);
+        }
+    trace.mark("hits: whole-target sweeps counted");
+    // ---- the place of every read in the output: counts per query, the first maxHits stored, forward strand first ----
+    std::vector<long long> cnt((size_t)N), base((size_t)N), stored((size_t)N);
+    be->d2h(cnt.data(), dPairCount.p, (size_t)N * sizeof(long long));
+    stats.d2hBytes += 8LL * N;
+    const int perQuery = p->strands ? 2 : 1;
+    out->counts = static_cast<long long*>(malloc(sizeof(long long) * (size_t)std::max(Q, 1)));
+    out->offsets = static_cast<long long*>(malloc(sizeof(long long) * ((size_t)Q + 1)));
+    if (!out->counts || !out->offsets) throw std::runtime_error("out of memory for the hit lists");
+    long long S = 0;
+    for (int q = 0; q < Q; ++q) {
+        long long total = 0, left = maxHits;
+        out->offsets[q] = S;
+        for (int s = 0; s < perQuery; ++s) {
+            const int pair = q * perQuery + s;
+            const long long st = std::min(cnt[(size_t)pair], std::max(left, 0LL));
+            base[(size_t)pair] = S;
+            stored[(size_t)pair] = st;
+            S += st;
+            left -= st;
+            total += cnt[(size_t)pair];
+        }
+        out->counts[q] = total;
+    }
+    out->offsets[Q] = S;
+    out->numQueries = Q;
+    out->columns = static_cast<int*>(malloc(sizeof(int) * (size_t)std::max(S, 1LL)));
+    out->scores = static_cast<int*>(malloc(sizeof(int) * (size_t)std::max(S, 1LL)));
+    if (p->strands) out->strands = static_cast<unsigned char*>(malloc((size_t)std::max(S, 1LL)));
+    if (!out->columns || !out->scores || (p->strands && !out->strands)) throw std::runtime_error("out of memory for the hit lists");
+    if (p->strands)
+        for (int pair = 0; pair < N; ++pair) memset(out->strands + base[(size_t)pair], pair & 1, (size_t)stored[(size_t)pair]);
+    trace.mark("hits: placed");
+    if (S == 0) return;
+    // ---- fill pass: only the jobs that store something are swept again ----
+    DevBuf<long long> dBase(be, (size_t)N), dStored(be, (size_t)N);
+    dBase.upload(base.data(), (size_t)N);
+    dStored.upload(stored.data(), (size_t)N);
+    DevBuf<int> dCols(be, (size_t)S), dScores(be, (size_t)S);
+    for (size_t ri = 0; ri < runs.size(); ++ri) {
+        HitRun& r = *runs[ri];
+        if (r.numJobs <= 0) continue;
+        const int g = (int)r.pairs.size();
+        r.dAt.alloc(be, (size_t)r.numJobs);
+        r.dRoom.alloc(be, (size_t)r.numJobs);
+        HitPlaceParams hp;
+        memset(&hp, 0, sizeof(hp));
+        hp.plan = ri < seedRuns ? r.dPlan.p : nullptr;
+        hp.chunks = r.chunks;
+        hp.numReads = g;
+        hp.readList = r.dList.p;
+        hp.count = r.dCount.p;
+        hp.pairBase = dBase.p;
+        hp.pairStored = dStored.p;
+        hp.at = r.dAt.p;
+        hp.room = r.dRoom.p;
+        be->launch_hits_place(hp);
+        const HitParams h{nullptr, r.dAt.p, r.dRoom.p, dCols.p, dScores.p};
+        if (ri < seedRuns) {
+            be->launch_k1w_hits(window_params(tg, r.jobs, r.numJobs), h, r.nw);
+        } else {
+            kp.readList = r.dList.p;
+            kp.kInit = r.dK.p;
+            kp.numReads = g;
+            kp.chunks = r.chunks;
+            kp.chunkLen = r.chunkLen;
+            kp.halo = 64 * r.nw;
+            be->launch_k1_hits(kp, h, r.nw);
+        }
+    }
+    dCols.download(out->columns, (size_t)S);
+    dScores.download(out->scores, (size_t)S);
+    stats.d2hBytes += 8 * S;
+    trace.mark("hits: filled");
 }
 }  // namespace eb

@@ -91,6 +91,41 @@ EDLIB_API EdlibB200Batch* edlibB200BatchPrepareStrands(const char* const* querie
  * prepared with edlibB200BatchPrepareStrands, or one that was not computed. */
 EDLIB_API int edlibB200BatchStrands(EdlibB200Batch* batch, unsigned char* strands);
 
+/* Every end location of each query within k edits of one shared target (HW mode).
+ *
+ * D(c), for a query q of m symbols and the target T of n symbols, is the HW last row at column c: the least edit
+ * distance between q and any substring of T that ends at c, the empty substring included.  The hits of q are all pairs
+ * (c, D(c)) with 0 <= c < n and D(c) <= k, in ascending c (column -1 is never reported; with k >= m every column is a
+ * hit).  So when edlibAlign(q, T, HW, k) gives a distance d >= 0, the least hit score is d and the columns scoring d
+ * are its endLocations (without a leading -1); when it gives -1 there are no hits.
+ *
+ * bothStrands != 0: rc(q) (the complement table of edlibB200AlignBatchStrands) is searched as well, with no pruning
+ * between the strands; its hits follow the forward ones and carry strand 1.
+ *
+ * counts[i] is the exact number of hits of query i over the searched strands; the first min(counts[i],
+ * maxHitsPerQuery) of them, in the order above, are stored at [offsets[i], offsets[i+1]) of columns / scores /
+ * strands (maxHitsPerQuery = 0: counts only).  Memory for stored hits is bounded by their number.
+ *
+ * Accepted: 1 <= queryLengths[i] <= 256, targetLength >= 1, config.k >= 0, config.mode == EDLIB_MODE_HW,
+ * config.task == EDLIB_TASK_DISTANCE, any additional equalities, maxHitsPerQuery >= 0.  Anything else returns
+ * EDLIB_STATUS_ERROR with a message in edlibB200LastError and *hits left empty; on success the arrays are malloc'd
+ * and edlibB200FreeHits releases them.  edlibB200LastStats: filterWindows = seed windows planned, filterDecided =
+ * query-strands whose hits came from seed windows, filterFallback = query-strands swept over the whole target. */
+typedef struct {
+    int numQueries;
+    long long* counts;      /* numQueries: hits found per query (all searched strands), may exceed what is stored */
+    long long* offsets;     /* numQueries + 1: stored hits of query i are [offsets[i], offsets[i+1]) */
+    int* columns;           /* end column of each stored hit */
+    int* scores;            /* D(column) */
+    unsigned char* strands; /* 0 / 1 per stored hit; NULL unless both strands were searched */
+} EdlibB200Hits;
+
+EDLIB_API int edlibB200FindHits(const char* const* queries, const int* queryLengths, int numQueries,
+                                const char* target, int targetLength, const EdlibAlignConfig config,
+                                int bothStrands, long long maxHitsPerQuery, EdlibB200Hits* hits);
+/* Frees the arrays of edlibB200FindHits and clears the struct. */
+EDLIB_API void edlibB200FreeHits(EdlibB200Hits* hits);
+
 /* A target kept resident on the device.  edlibAlignBatch calls of read sets (HW, short queries, plain equality) whose
  * targets[i] all equal (target, targetLength) of a live handle skip the target's upload, its encoding and the build of
  * its seed index: a caller that aligns many batches to one genome pays them once.  The bytes at `target` must not
