@@ -113,27 +113,42 @@ def align_batch(queries, targets, mode="NW", task="distance", k=-1, additionalEq
 align_many = align_batch  # the name SURVEY.md 8f proposes for the batched binding entry
 
 
-def find_hits(queries, target, k, strands="forward", max_hits=None, additionalEqualities=None):
+def find_hits(queries, target, k, strands="forward", max_hits=None, additionalEqualities=None, task="distance"):
     """Every place where each query occurs in `target` with at most k edits (HW mode; queries of 1..256 symbols).
 
     Returns one dict per query: {"count": number of hits, "hits": [(column, score), ...]}, where the hits are every
     end column c of `target` whose best alignment of the query ending there has score <= k, in ascending columns.
     At most `max_hits` hits are listed per query (None: all); "count" is always the full number.
     strands="both": the reverse complement is searched too; its hits follow the forward ones and every hit becomes
-    (column, score, "+" or "-").  The sequence rules are those of `align_batch`."""
+    (column, score, "+" or "-").  The sequence rules are those of `align_batch`.
+
+    task="locations" adds "starts", one per listed hit: the first target column of the hit's alignment (the smallest
+    start whose alignment to [start, column] still has the hit's score).  task="path" adds "cigars" as well: the
+    extended CIGAR of that alignment, as `align(..., task="path")` gives it; a "-" hit's CIGAR aligns the reverse
+    complement.  For the columns of a query's least score these are exactly `align(query, target, "HW", task, k)`'s
+    locations, and its CIGAR is the one of the first of them."""
     if strands not in ("forward", "both"):
         raise ValueError("strands must be 'forward' or 'both'")
+    if task not in ("distance", "locations", "path"):
+        raise ValueError("task must be 'distance', 'locations' or 'path'")
     queries = list(queries)
     if strands == "both" and not all(_is_plain(s) for s in queries + [target]):
         raise ValueError("strands='both' needs bytes or ASCII str sequences")
     mapped, eqs = _map_to_bytes(queries + [target], additionalEqualities)
     both = strands == "both"
-    st, res = library().find_hits(mapped[:-1], mapped[-1], k, both, (1 << 62) if max_hits is None else max_hits, eqs)
+    cap = (1 << 62) if max_hits is None else max_hits
+    lib = library()
+    if task == "distance":
+        st, res = lib.find_hits(mapped[:-1], mapped[-1], k, both, cap, eqs)
+    else:
+        st, res = lib.find_hit_alignments(mapped[:-1], mapped[-1], k, both, cap, eqs, TASKS[task])
     if st != EDLIB_STATUS_OK:
-        raise Exception("There was an error. (" + library().lib.edlibB200LastError().decode() + ")")
-    if both:
-        for r in res:
+        raise Exception("There was an error. (" + lib.lib.edlibB200LastError().decode() + ")")
+    for r in res:
+        if both:
             r["hits"] = [(c, s, "-" if d else "+") for c, s, d in r["hits"]]
+        if "alignments" in r:
+            r["cigars"] = [lib.cigar(a, EDLIB_CIGAR_EXTENDED) for a in r.pop("alignments")]
     return res
 
 

@@ -39,8 +39,13 @@ class Hits(C.Structure):                  # include/edlib_b200.h EdlibB200Hits (
                 ("columns", C.POINTER(C.c_int)), ("scores", C.POINTER(C.c_int)), ("strands", C.POINTER(C.c_ubyte))]
 
 
+class HitAlignments(C.Structure):         # include/edlib_b200.h EdlibB200HitAlignments (72 bytes)
+    _fields_ = [("hits", Hits), ("starts", C.POINTER(C.c_int)), ("alignmentOffsets", C.POINTER(C.c_longlong)),
+                ("alignments", C.POINTER(C.c_ubyte))]
+
+
 assert C.sizeof(EqualityPair) == 2 and C.sizeof(AlignConfig) == 32 and C.sizeof(AlignResult) == 48
-assert C.sizeof(Hits) == 48
+assert C.sizeof(Hits) == 48 and C.sizeof(HitAlignments) == 72
 
 
 def make_config(k=-1, mode=EDLIB_MODE_NW, task=EDLIB_TASK_DISTANCE, equalities=None):
@@ -169,6 +174,42 @@ class EdlibLib:
             hits = list(zip(cols, scores, h.strands[a:b])) if both else list(zip(cols, scores))
             out.append({"count": h.counts[i], "hits": hits})
         self.lib.edlibB200FreeHits(C.byref(h))
+        return st, out
+
+    def find_hit_alignments(self, queries, target, k, both=False, max_hits=(1 << 62), equalities=None,
+                            task=EDLIB_TASK_DISTANCE, mode=EDLIB_MODE_HW):
+        """edlibB200FindHitAlignments over one shared target.  Returns (status, [dict]) as find_hits; with task LOC /
+        PATH each dict also has "starts" (one per stored hit), with PATH "alignments" (bytes of EDLIB_EDOP_* codes,
+        one per stored hit); status != 0: (status, None)."""
+        fn = self.lib.edlibB200FindHitAlignments
+        fn.restype = C.c_int
+        fn.argtypes = [C.POINTER(C.c_char_p), C.POINTER(C.c_int), C.c_int, C.c_char_p, C.c_int, AlignConfig, C.c_int,
+                       C.c_longlong, C.POINTER(HitAlignments)]
+        self.lib.edlibB200FreeHitAlignments.restype = None
+        self.lib.edlibB200FreeHitAlignments.argtypes = [C.POINTER(HitAlignments)]
+        n = len(queries)
+        cfg, keep = make_config(k, mode, task, equalities)
+        qptr = (C.c_char_p * max(n, 1))(*queries)
+        qlen = (C.c_int * max(n, 1))(*[len(q) for q in queries])
+        a = HitAlignments()
+        st = fn(qptr, qlen, n, target, len(target), cfg, 1 if both else 0, max_hits, C.byref(a))
+        del keep
+        if st != EDLIB_STATUS_OK:
+            return st, None
+        h = a.hits
+        out = []
+        for i in range(n):
+            lo, hi = h.offsets[i], h.offsets[i + 1]
+            cols, scores = h.columns[lo:hi], h.scores[lo:hi]
+            r = {"count": h.counts[i],
+                 "hits": list(zip(cols, scores, h.strands[lo:hi])) if both else list(zip(cols, scores))}
+            if a.starts:
+                r["starts"] = a.starts[lo:hi]
+            if a.alignments:
+                off, base = a.alignmentOffsets, C.cast(a.alignments, C.c_void_p).value
+                r["alignments"] = [C.string_at(base + off[j], off[j + 1] - off[j]) for j in range(lo, hi)]
+            out.append(r)
+        self.lib.edlibB200FreeHitAlignments(C.byref(a))
         return st, out
 
     def _run_batch(self, call, queries, targets, k, mode, task, equalities):

@@ -25,6 +25,7 @@ void host_parallel_ranges(size_t n, size_t grain, const std::function<void(size_
 void free_result_arrays(EdlibAlignResult* results, size_t lo, size_t hi);  // eb_engine.cpp: frees and clears them
 void fail_results(EdlibAlignResult* results, int n);  // eb_engine.cpp: error results (status, distance -1, no arrays)
 void free_hits(EdlibB200Hits* h);  // eb_engine.cpp: frees the arrays of a hit list and clears it
+void free_hit_alignments(EdlibB200HitAlignments* h);  // eb_engine.cpp: ... and the starts / scripts of its hits
 Backend* create_backend(std::string* err);  // provided by the backend object linked into this library
 int select_device(int device, std::string* err);  // 0 on success
 }
@@ -462,43 +463,51 @@ EDLIB_API void edlibB200FreeCigars(char** cigars, int n) {
     eb::host_parallel_ranges((size_t)n, 16384, free_range);
 }
 
-// What edlibB200FindHits refuses (include/edlib_b200.h), or nullptr.
-static const char* hits_input_error(const char* const* queries, const int* queryLengths, int numQueries, const char* target,
-                                    int targetLength, const EdlibAlignConfig& config, int bothStrands, long long maxHits) {
-    if (numQueries < 0) return "edlibB200FindHits: numQueries < 0";
-    if (numQueries > 0 && (!queries || !queryLengths)) return "edlibB200FindHits: no queries";
-    if (bothStrands && numQueries > 0x3fffffff) return "edlibB200FindHits: too many queries for both strands";
-    if (!target || targetLength < 1) return "edlibB200FindHits: the target must have at least one symbol";
-    if (config.mode != EDLIB_MODE_HW) return "edlibB200FindHits: mode must be EDLIB_MODE_HW";
-    if (config.task != EDLIB_TASK_DISTANCE) return "edlibB200FindHits: task must be EDLIB_TASK_DISTANCE";
-    if (config.k < 0) return "edlibB200FindHits: k must be >= 0";
-    if (maxHits < 0) return "edlibB200FindHits: maxHitsPerQuery must be >= 0";
-    if (config.additionalEqualitiesLength > 0 && !config.additionalEqualities) return "edlibB200FindHits: no equality pairs";
+// What edlibB200FindHits (alignments == false) / edlibB200FindHitAlignments refuse (include/edlib_b200.h), or "".
+static std::string hits_input_error(const char* entry, bool alignments, const char* const* queries, const int* queryLengths,
+                                    int numQueries, const char* target, int targetLength, const EdlibAlignConfig& config,
+                                    int bothStrands, long long maxHits) {
+    const std::string at = std::string(entry) + ": ";
+    if (numQueries < 0) return at + "numQueries < 0";
+    if (numQueries > 0 && (!queries || !queryLengths)) return at + "no queries";
+    if (bothStrands && numQueries > 0x3fffffff) return at + "too many queries for both strands";
+    if (!target || targetLength < 1) return at + "the target must have at least one symbol";
+    if (config.mode != EDLIB_MODE_HW) return at + "mode must be EDLIB_MODE_HW";
+    if (!alignments && config.task != EDLIB_TASK_DISTANCE) return at + "task must be EDLIB_TASK_DISTANCE";
+    if (alignments && config.task != EDLIB_TASK_DISTANCE && config.task != EDLIB_TASK_LOC && config.task != EDLIB_TASK_PATH)
+        return at + "task must be EDLIB_TASK_DISTANCE, EDLIB_TASK_LOC or EDLIB_TASK_PATH";
+    if (config.k < 0) return at + "k must be >= 0";
+    if (maxHits < 0) return at + "maxHitsPerQuery must be >= 0";
+    if (config.additionalEqualitiesLength > 0 && !config.additionalEqualities) return at + "no equality pairs";
     for (int i = 0; i < numQueries; ++i)
-        if (!queries[i] || queryLengths[i] < 1 || queryLengths[i] > 256) return "edlibB200FindHits: query lengths must be 1 .. 256";
-    return nullptr;
+        if (!queries[i] || queryLengths[i] < 1 || queryLengths[i] > 256) return at + "query lengths must be 1 .. 256";
+    return std::string();
 }
 
-EDLIB_API int edlibB200FindHits(const char* const* queries, const int* queryLengths, int numQueries, const char* target,
-                                int targetLength, const EdlibAlignConfig config, int bothStrands, long long maxHitsPerQuery,
-                                EdlibB200Hits* hits) {
+// Both hit entries: `out` (never NULL here) is cleared, then filled on success; on failure nothing stays allocated.
+static int find_hits_entry(const char* entry, bool alignments, bool outNull, const char* const* queries,
+                           const int* queryLengths, int numQueries, const char* target, int targetLength,
+                           const EdlibAlignConfig& config, int bothStrands, long long maxHitsPerQuery,
+                           EdlibB200HitAlignments* out) {
     std::lock_guard<std::mutex> lock(g_mu);
     eb::Engine* e = engine_locked();
-    if (hits) memset(hits, 0, sizeof(*hits));
+    memset(out, 0, sizeof(*out));
     if (!e) return EDLIB_STATUS_ERROR;  // no usable device: there is no CPU path
     t_lastEngine = e;
-    const char* bad = hits ? hits_input_error(queries, queryLengths, numQueries, target, targetLength, config, bothStrands,
-                                              maxHitsPerQuery)
-                           : "edlibB200FindHits: hits is NULL";
-    if (bad) {
+    const std::string bad = outNull ? std::string(entry) + (alignments ? ": out is NULL" : ": hits is NULL")
+                                    : hits_input_error(entry, alignments, queries, queryLengths, numQueries, target,
+                                                       targetLength, config, bothStrands, maxHitsPerQuery);
+    if (!bad.empty()) {
         e->lastError = bad;
         return EDLIB_STATUS_ERROR;
     }
     if (numQueries == 0) {
-        hits->offsets = static_cast<long long*>(calloc(1, sizeof(long long)));
-        hits->counts = static_cast<long long*>(malloc(sizeof(long long)));
-        if (hits->offsets && hits->counts) return EDLIB_STATUS_OK;
-        eb::free_hits(hits);
+        out->hits.offsets = static_cast<long long*>(calloc(1, sizeof(long long)));
+        out->hits.counts = static_cast<long long*>(malloc(sizeof(long long)));
+        if (config.task == EDLIB_TASK_PATH) out->alignmentOffsets = static_cast<long long*>(calloc(1, sizeof(long long)));
+        if (out->hits.offsets && out->hits.counts && (config.task != EDLIB_TASK_PATH || out->alignmentOffsets))
+            return EDLIB_STATUS_OK;
+        eb::free_hit_alignments(out);
         e->lastError = "out of memory for the hit lists";
         return EDLIB_STATUS_ERROR;
     }
@@ -506,11 +515,33 @@ EDLIB_API int edlibB200FindHits(const char* const* queries, const int* queryLeng
     const std::vector<int> targetLengths((size_t)numQueries, targetLength);
     eb::BatchInput in{queries, queryLengths, targets.data(), targetLengths.data(), numQueries, config};
     in.strands = bothStrands != 0;
-    return e->find_hits(in, maxHitsPerQuery, hits);
+    return e->find_hits(in, maxHitsPerQuery, out);
+}
+
+EDLIB_API int edlibB200FindHits(const char* const* queries, const int* queryLengths, int numQueries, const char* target,
+                                int targetLength, const EdlibAlignConfig config, int bothStrands, long long maxHitsPerQuery,
+                                EdlibB200Hits* hits) {
+    EdlibB200HitAlignments out;
+    const int st = find_hits_entry("edlibB200FindHits", false, !hits, queries, queryLengths, numQueries, target,
+                                   targetLength, config, bothStrands, maxHitsPerQuery, &out);
+    if (hits) *hits = out.hits;  // task DISTANCE: nothing else was allocated
+    return st;
 }
 
 EDLIB_API void edlibB200FreeHits(EdlibB200Hits* hits) {
     if (hits) eb::free_hits(hits);
+}
+
+EDLIB_API int edlibB200FindHitAlignments(const char* const* queries, const int* queryLengths, int numQueries,
+                                         const char* target, int targetLength, const EdlibAlignConfig config,
+                                         int bothStrands, long long maxHitsPerQuery, EdlibB200HitAlignments* out) {
+    EdlibB200HitAlignments scratch;
+    return find_hits_entry("edlibB200FindHitAlignments", true, !out, queries, queryLengths, numQueries, target,
+                           targetLength, config, bothStrands, maxHitsPerQuery, out ? out : &scratch);
+}
+
+EDLIB_API void edlibB200FreeHitAlignments(EdlibB200HitAlignments* out) {
+    if (out) eb::free_hit_alignments(out);
 }
 
 EDLIB_API void edlibB200LastStats(EdlibB200Stats* s) {

@@ -406,6 +406,45 @@ struct HitPlaceParams {
     long long* at;           // hits_place: [job] -> HitParams::at
     int* room;               // hits_place: [job] -> HitParams::room
 };
+// Start locations and edit scripts of stored hits (edlibB200FindHitAlignments), one slice of stored hits at a time:
+// the lane kernel runs one reversed SHW sweep (start) and one matrix-storing NW sweep + traceback (script) per hit of
+// word class nw; `stage` selects the per-item function of hit_res_kernel.  Hit h of the slice is stored hit
+// firstHit + h; its pair is the last pair whose first stored slot is <= firstHit + h.
+enum HitResStage : int {
+    HR_FLAG = 0,        // item = hit h: cnt[h] = 1 if its query is of word class nw                                -> scan
+    HR_LOC_JOBS = 1,    // item = hit h of the class: LJob j = cnt[h] of the reversed SHW sweep ending at its column
+    HR_LOC_APPLY = 2,   // item = job j: starts[h] = column - last column of the sweep's best (ref cpp:260), best == score
+    HR_PATH_JOBS = 3,   // item = hit h of the class: LJob (storing NW) + TbJob j = cnt[h] over [starts[h], column]
+    HR_PATH_LEN = 4,    // item = job j: len[h] = ops of its edit script, NW score == score                         -> scan
+    HR_PATH_COPY = 5,   // item = job j: edit script into the slice's dense pool at len[h]
+};
+struct HitResParams {
+    int stage;
+    int nw;                  // word class handled by this launch
+    int numItems;            // hits of the slice (HR_FLAG, HR_*_JOBS) or jobs of the class (the others)
+    long long firstHit;      // stored slot of hit 0 of the slice
+    int numPairs;
+    const long long* pairBase;  // [numPairs] first stored slot of each pair (non-decreasing)
+    const int* qlen;         // [pair]
+    const uint64_t* qoff;    // [pair]
+    uint64_t tOff;           // offset of the shared target in the packed buffer
+    const int* cols;         // [stored hit] end column
+    const int* scores;       // [stored hit] D(column)
+    int* cnt;                // [hits + 1] flags, then their exclusive prefix sums: job of hit h is cnt[h]
+    LJob* jobs;
+    int* jobHit;             // [job] hit of the job inside the slice
+    const Rec* recs;         // [job] outcome of the lane sweeps
+    int* starts;             // [hits] start location of each hit
+    TbJob* tb;
+    uint64_t matStride;      // HR_PATH_JOBS: U2 entries reserved per job
+    uint64_t opsStride;      // bytes reserved per job for its traceback
+    const uint8_t* ops;      // traceback output (opsStride per job), opsStart / opsLen per job
+    const int* opsStart;
+    const int* opsLen;
+    int* len;                // [hits + 1] script length of each hit, then their exclusive prefix sums
+    uint8_t* pool;           // dense scripts of the slice, in hit order
+    int* err;                // set to 1 when a sweep disagrees with the score of its hit
+};
 
 // ---------------------------------------------------------------------------------------------
 // Start locations and alignment paths of short queries (<= 256 rows) WITHOUT the host in the loop: the jobs of the

@@ -1507,6 +1507,106 @@ EB_HD void res_item(const ResParams& p, int i) {
     }
 }
 
+// Start locations / edit scripts of stored hits (eb_common.h: HitResParams).  The rules are those of a single hit
+// of edlibAlign (ref cpp:228-289) applied to each hit (column c, score s) on its own: the start is c minus the last
+// column of best score s of the reversed SHW sweep over the last m + s columns, the script that of the NW alignment of
+// the query to [start, c].
+EB_HD int hit_res_pair(const HitResParams& p, long long slot) {  // last pair whose first slot is <= slot
+    int lo = 0, hi = p.numPairs - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (p.pairBase[mid] <= slot) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+
+EB_HD void hit_res_item(const HitResParams& p, int i) {
+    switch (p.stage) {
+        case HR_FLAG: {
+            const int m = p.qlen[hit_res_pair(p, p.firstHit + i)];
+            p.cnt[i] = (m + 31) / 32 == p.nw ? 1 : 0;
+            break;
+        }
+        case HR_LOC_JOBS: {
+            if (p.cnt[i + 1] == p.cnt[i]) break;
+            const int j = p.cnt[i];
+            const long long slot = p.firstHit + i;
+            const int pair = hit_res_pair(p, slot);
+            const int c = p.cols[slot], s = p.scores[slot], m = p.qlen[pair];
+            LJob J;
+            J.qOff = p.qoff[pair];
+            J.tOff = p.tOff + (uint64_t)c;  // first symbol read, walking backwards
+            J.matOff = 0;
+            J.m = m;
+            const long long span = (long long)m + s;  // a start further back costs more than s
+            J.n = (int)((long long)c + 1 < span ? (long long)c + 1 : span);
+            J.kInit = s + 1;
+            J.trackFrom = 0;
+            p.jobs[j] = J;
+            p.jobHit[j] = i;
+            break;
+        }
+        case HR_LOC_APPLY: {
+            const int h = p.jobHit[i];
+            const long long slot = p.firstHit + h;
+            const Rec r = p.recs[i];
+            if (r.cnt <= 0 || r.best != p.scores[slot]) *p.err = 1;
+            p.starts[h] = p.cols[slot] - r.last;  // ref cpp:260
+            break;
+        }
+        case HR_PATH_JOBS: {
+            if (p.cnt[i + 1] == p.cnt[i]) break;
+            const int j = p.cnt[i];
+            const long long slot = p.firstHit + i;
+            const int pair = hit_res_pair(p, slot);
+            const int st = p.starts[i];
+            LJob J;
+            J.qOff = p.qoff[pair];
+            J.tOff = p.tOff + (uint64_t)st;
+            J.matOff = (uint64_t)(j / 32) * 32u * p.matStride + (uint64_t)(j % 32);  // interleaved by 32 jobs (LParams::matStep)
+            J.m = p.qlen[pair];
+            J.n = p.cols[slot] - st + 1;
+            J.kInit = 0;
+            J.trackFrom = 0;
+            if (J.n < 1 || (uint64_t)J.n * (uint64_t)p.nw > p.matStride || (uint64_t)(J.m + J.n) > p.opsStride) {
+                *p.err = 1;  // cannot happen: 1 <= c - start + 1 <= m + s, which the strides cover
+                J.m = 0;
+                J.n = 0;
+            }
+            p.jobs[j] = J;
+            TbJob T;
+            T.matOff = J.matOff;
+            T.qOff = J.qOff;
+            T.peqOff = ~0ull;
+            T.tOff = J.tOff;
+            T.outOff = (uint64_t)j * p.opsStride;
+            T.m = J.m;
+            T.n = J.n;
+            T.nWp = p.nw;
+            T.rsv = 0;
+            p.tb[j] = T;
+            p.jobHit[j] = i;
+            break;
+        }
+        case HR_PATH_LEN: {
+            const int h = p.jobHit[i];
+            if (p.jobs[i].n <= 0 || p.recs[i].best != p.scores[p.firstHit + h]) *p.err = 1;
+            p.len[h] = p.opsLen[i];
+            break;
+        }
+        case HR_PATH_COPY: {
+            const int h = p.jobHit[i];
+            const int len = p.len[h + 1] - p.len[h];
+            const uint8_t* src = p.ops + (uint64_t)i * p.opsStride + (uint64_t)p.opsStart[i];
+            uint8_t* dst = p.pool + p.len[h];
+            for (int x = 0; x < len; ++x) dst[x] = src[x];
+            break;
+        }
+        default: break;
+    }
+}
+
 // =============================================================================================
 // B -- k-banded NW sweep of a LONG query, one alignment per THREAD (ref myersCalcEditDistanceNW cpp:730-928 with
 // its Ukkonen band, cpp:755, 799-830).  The thread holds a window of NW = 4*NB words (32*NW rows) of the column in

@@ -917,19 +917,29 @@ void free_hits(EdlibB200Hits* h) {
     memset(h, 0, sizeof(*h));
 }
 
+void free_hit_alignments(EdlibB200HitAlignments* h) {
+    free_hits(&h->hits);
+    free(h->starts);
+    free(h->alignmentOffsets);
+    free(h->alignments);
+    memset(h, 0, sizeof(*h));
+}
+
 // The grouped batch of every query against the one target (a strand batch for both strands), then the hits pass
 // instead of the distance pass.
-int Engine::find_hits(const BatchInput& in, long long maxHits, EdlibB200Hits* out) {
+int Engine::find_hits(const BatchInput& in, long long maxHits, EdlibB200HitAlignments* out) {
     Prepared* p = nullptr;
     stats = EngineStats();
     statsPending_ = false;
     memset(out, 0, sizeof(*out));
     try {
-        p = prepare(in);
+        BatchInput din = in;  // the batch itself is that of edlibB200FindHits: the task only adds a stage
+        din.config.task = EDLIB_TASK_DISTANCE;
+        p = prepare(din);
         be_->reset_timing();
         {
             Pass ps(*this, be_, p);
-            ps.hits(maxHits, out);
+            ps.hits(maxHits, in.config.task, out);
         }
         be_->sync_all();
         be_->release_marks();
@@ -941,7 +951,7 @@ int Engine::find_hits(const BatchInput& in, long long maxHits, EdlibB200Hits* ou
         lastError = e.what();
         quiesce();
         if (p) release(p);
-        free_hits(out);
+        free_hit_alignments(out);
         return EDLIB_STATUS_ERROR;
     }
 }

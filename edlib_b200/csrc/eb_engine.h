@@ -91,6 +91,8 @@ struct Backend {
     virtual void launch_k1_hits(const K1Params&, const HitParams&, int /*nw32*/) { no_kernel("k1_hits"); }
     virtual void launch_hits_total(const HitPlaceParams&) { no_kernel("hits_total"); }
     virtual void launch_hits_place(const HitPlaceParams&) { no_kernel("hits_place"); }
+    // start locations / edit scripts of stored hits (eb_common.h: HitResParams)
+    virtual void launch_hit_res(const HitResParams&) { no_kernel("hit_res"); }
     [[noreturn]] static void no_kernel(const char* name) {
         throw std::runtime_error(std::string(name) + ": no such kernel on this backend");
     }
@@ -194,10 +196,11 @@ public:
     // One-shot streamed path for large HW batches of short reads over one shared target (eb_engine.cpp): returns
     // false when the batch is not of that shape (nothing done), throws on failure.
     bool align_streamed(const BatchInput& in, EdlibAlignResult* results);
-    // edlibB200FindHits: every end column within config.k of every query over the one shared target (in.strands: of its
-    // reverse complement too), at most maxHits stored per query.  `out` is filled with malloc'd arrays; on failure
-    // nothing stays allocated.  Returns EDLIB_STATUS_OK / EDLIB_STATUS_ERROR.
-    int find_hits(const BatchInput& in, long long maxHits, EdlibB200Hits* out);
+    // edlibB200FindHits / edlibB200FindHitAlignments: every end column within config.k of every query over the one
+    // shared target (in.strands: of its reverse complement too), at most maxHits stored per query; config.task LOC /
+    // PATH adds the start location / edit script of every stored hit.  `out` is filled with malloc'd arrays; on
+    // failure nothing stays allocated.  Returns EDLIB_STATUS_OK / EDLIB_STATUS_ERROR.
+    int find_hits(const BatchInput& in, long long maxHits, EdlibB200HitAlignments* out);
 
     void finish_stats();  // fills the device-time fields of `stats` for the last pass (on demand)
 

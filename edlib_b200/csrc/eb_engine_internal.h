@@ -722,8 +722,13 @@ struct Pass {
     // Runs instead of the distance pass: every end column scoring <= k of every pair over the batch's one target, into
     // `out` (malloc'd arrays; the two pairs of a read of a strand batch share its cap, forward first).  A pair takes the
     // seed windows of the first level whose threshold reaches k, or the whole-target sweep (no such level, saturated
-    // plan, repeats, short target, equality table); both count, place, then fill.
-    void hits(long long maxHits, EdlibB200Hits* out);
+    // plan, repeats, short target, equality table); both count, place, then fill.  task LOC / PATH: then the start
+    // location / edit script of every stored hit (hit_alignments).
+    void hits(long long maxHits, int task, EdlibB200HitAlignments* out);
+    // Start locations (and, task PATH, edit scripts) of the S stored hits in dCols / dScores, whose pairs start at
+    // dBase: lane sweeps per word class over slices of stored hits, jobs built on the device (eb_core.h: hit_res_item).
+    void hit_alignments(int task, long long S, const std::vector<long long>& stored, const long long* dBase,
+                        const int* dCols, const int* dScores, EdlibB200HitAlignments* out);
     // The K1W launch over the first numJobs jobs (or as many as *jobs.count says, numJobs < 0), records not set.
     K1WParams window_params(const Target& tg, const WinJobs& jobs, int numJobs) const;
 

@@ -359,6 +359,10 @@ __global__ void hits_place_kernel(const HitPlaceParams p) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < p.numReads) hits_place_item(p, i);
 }
+__global__ void hit_res_kernel(const HitResParams p) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < p.numItems) hit_res_item(p, i);
+}
 
 // L: one alignment per thread over its own target (eb_core.h: lane_job).
 template <int NW, int MODE, bool REV, bool STORE>
@@ -1001,6 +1005,9 @@ struct CudaBackend : Backend {
     }
     void launch_hits_place(const HitPlaceParams& p) override {
         if (p.numReads > 0) launch("hits_place", hits_place_kernel, (p.numReads + 255) / 256, 256, 0, p);
+    }
+    void launch_hit_res(const HitResParams& p) override {
+        if (p.numItems > 0) launch("hit_res", hit_res_kernel, (p.numItems + 255) / 256, 256, 0, p);
     }
     void launch_lane(const LParams& p, int nw, int mode, bool rev, bool store) override {
         int block = 128;

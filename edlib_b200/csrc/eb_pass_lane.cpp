@@ -956,7 +956,8 @@ struct HitRun {
 constexpr int HIT_RUN_READS = 1 << 18;  // reads per launch group (bounds the per-job arrays of a whole-target sweep)
 }  // namespace
 
-void Pass::hits(long long maxHits, EdlibB200Hits* out) {
+void Pass::hits(long long maxHits, int task, EdlibB200HitAlignments* outAln) {
+    EdlibB200Hits* out = &outAln->hits;
     if (p->tg.size() != 1) throw std::runtime_error("internal: hits need one shared target");
     const Target& tg = p->tg[0];
     const int n = tg.len;
@@ -1111,7 +1112,10 @@ void Pass::hits(long long maxHits, EdlibB200Hits* out) {
     if (p->strands)
         for (int pair = 0; pair < N; ++pair) memset(out->strands + base[(size_t)pair], pair & 1, (size_t)stored[(size_t)pair]);
     trace.mark("hits: placed");
-    if (S == 0) return;
+    if (S == 0) {
+        if (task != EDLIB_TASK_DISTANCE) hit_alignments(task, 0, stored, nullptr, nullptr, nullptr, outAln);
+        return;
+    }
     // ---- fill pass: only the jobs that store something are swept again ----
     DevBuf<long long> dBase(be, (size_t)N), dStored(be, (size_t)N);
     dBase.upload(base.data(), (size_t)N);
@@ -1152,5 +1156,158 @@ void Pass::hits(long long maxHits, EdlibB200Hits* out) {
     dScores.download(out->scores, (size_t)S);
     stats.d2hBytes += 8 * S;
     trace.mark("hits: filled");
+    if (task != EDLIB_TASK_DISTANCE) hit_alignments(task, S, stored, dBase.p, dCols.p, dScores.p, outAln);
+}
+
+// Start locations and edit scripts of the stored hits.  The stored hits are cut into slices of consecutive slots whose
+// jobs (and, task PATH, stored matrices) fit tun.pathSliceBytes and whose scripts stay countable in an int; inside a
+// slice, each word class of the lane kernel gets its jobs from a flag scan over the slice's hits, the reversed SHW
+// sweeps give the starts, the matrix-storing NW sweeps + traceback the scripts, and the scripts of the slice are
+// compacted in hit order into one dense pool that comes back in one copy.
+namespace {
+struct HitPathClass {  // what the script copy of one word class of a slice needs after its sweeps
+    int nw = 0, jobs = 0;
+    uint64_t opsStride = 0;
+    DevBuf<int> dJobHit, dOpsStart, dOpsLen;
+    DevBuf<uint8_t> dOps;
+};
+}  // namespace
+
+void Pass::hit_alignments(int task, long long S, const std::vector<long long>& stored, const long long* dBase,
+                           const int* dCols, const int* dScores, EdlibB200HitAlignments* out) {
+    const bool path = task == EDLIB_TASK_PATH;
+    out->starts = static_cast<int*>(malloc(sizeof(int) * (size_t)std::max(S, 1LL)));
+    if (path) out->alignmentOffsets = static_cast<long long*>(malloc(sizeof(long long) * ((size_t)S + 1)));
+    if (!out->starts || (path && !out->alignmentOffsets)) throw std::runtime_error("out of memory for the hit alignments");
+    if (path) out->alignmentOffsets[0] = 0;
+    if (S == 0) {
+        if (path && !(out->alignments = static_cast<unsigned char*>(malloc(1))))
+            throw std::runtime_error("out of memory for the hit alignments");
+        return;
+    }
+    unsigned classes = 0;  // word classes of the queries with stored hits
+    for (int pair = 0; pair < N; ++pair)
+        if (stored[(size_t)pair] > 0) classes |= 1u << ceil_div(p->qlen[pair], 32);
+    int maxNw = 0;
+    for (int nw = 1; nw <= 8; ++nw) {
+        if (!((classes >> nw) & 1u)) continue;
+        if (!runner.lane_ok(nw)) throw std::runtime_error("hit alignments: alphabet too large for the lane kernel");
+        maxNw = nw;
+    }
+    // a hit's target slice [start, c] has at most m + s <= min(2m, m + k) columns
+    auto maxPathN = [&](int nw) { return (uint64_t)std::min<long long>(64LL * nw, 32LL * nw + k); };
+    const uint64_t maxMat = maxPathN(maxNw) * (uint64_t)maxNw, maxOps = 32ull * maxNw + maxPathN(maxNw);
+    const size_t perHit = sizeof(LJob) + sizeof(Rec) + 6 * sizeof(int) +
+                          (path ? (size_t)maxMat * sizeof(U2) + 2 * (size_t)maxOps + sizeof(TbJob) + 3 * sizeof(int) : 0);
+    long long H = std::max<long long>(32, (long long)(tun.pathSliceBytes / perHit));
+    H = std::min(H, 1LL << 30);                                      // the flag scans count in an int
+    if (path) H = std::min(H, (long long)(0x7fffffff / maxOps) - 1);  // so do the script lengths
+    H = std::min(H, S);
+    const uint64_t tOff = p->tg[0].off;
+    DevBuf<int> dErr(be, 1);
+    be->zero(dErr.p, sizeof(int));
+    DevBuf<int> dCnt(be, (size_t)H + 1), dStart(be, (size_t)H), dLen(be, path ? (size_t)H + 1 : 1);
+    std::vector<int> lenScan(path ? (size_t)H + 1 : 0);
+    long long poolAt = 0;
+    for (long long lo = 0; lo < S; lo += H) {
+        const int span = (int)std::min(H, S - lo);
+        HitResParams hp;
+        memset(&hp, 0, sizeof(hp));
+        hp.firstHit = lo;
+        hp.numPairs = N;
+        hp.pairBase = dBase;
+        hp.qlen = p->dQlen.p;
+        hp.qoff = p->dQoff.p;
+        hp.tOff = tOff;
+        hp.cols = dCols;
+        hp.scores = dScores;
+        hp.cnt = dCnt.p;
+        hp.starts = dStart.p;
+        hp.len = dLen.p;
+        hp.err = dErr.p;
+        std::vector<std::unique_ptr<HitPathClass>> done;
+        for (int nw = 1; nw <= 8; ++nw) {
+            if (!((classes >> nw) & 1u)) continue;
+            hp.nw = nw;
+            hp.stage = HR_FLAG;
+            hp.numItems = span;
+            be->launch_hit_res(hp);
+            be->launch_scan(dCnt.p, span);
+            int J = 0;
+            be->d2h(&J, dCnt.p + span, sizeof(int));
+            if (J <= 0) continue;
+            std::unique_ptr<HitPathClass> c(new HitPathClass());
+            c->nw = nw;
+            c->jobs = J;
+            c->dJobHit.alloc(be, (size_t)J);
+            DevBuf<LJob> dJobs(be, (size_t)J);
+            DevBuf<Rec> dRecs(be, (size_t)J);
+            hp.jobs = dJobs.p;
+            hp.jobHit = c->dJobHit.p;
+            hp.recs = dRecs.p;
+            hp.stage = HR_LOC_JOBS;
+            be->launch_hit_res(hp);
+            const LParams lp{dJobs.p, J, p->dSeq.p, p->dSeq.p, p->ncodes, p->hasEq ? p->dEqtab.p : nullptr, dRecs.p, nullptr, 1};
+            be->launch_lane(lp, nw, MODE_SHW, true, false);
+            hp.stage = HR_LOC_APPLY;
+            hp.numItems = J;
+            be->launch_hit_res(hp);
+            if (!path) continue;
+            const uint64_t maxN = maxPathN(nw);
+            hp.matStride = maxN * (uint64_t)nw;
+            hp.opsStride = c->opsStride = 32ull * nw + maxN;
+            DevBuf<TbJob> dTb(be, (size_t)J);
+            DevBuf<U2> dMat(be, (size_t)ceil_div(J, 32) * 32 * hp.matStride);
+            c->dOps.alloc(be, (size_t)J * hp.opsStride);
+            c->dOpsStart.alloc(be, (size_t)J);
+            c->dOpsLen.alloc(be, (size_t)J);
+            hp.tb = dTb.p;
+            hp.stage = HR_PATH_JOBS;
+            hp.numItems = span;
+            be->launch_hit_res(hp);
+            const LParams sp{dJobs.p, J, p->dSeq.p, p->dSeq.p, p->ncodes, p->hasEq ? p->dEqtab.p : nullptr, dRecs.p, dMat.p, 32};
+            be->launch_lane(sp, nw, MODE_NW, false, true);
+            const TbParams tp{dTb.p, J, dMat.p, nullptr, p->dSeq.p, p->dSeq.p, p->hasEq ? p->dEqtab.p : nullptr, p->ncodes,
+                              c->dOps.p, c->dOpsStart.p, c->dOpsLen.p, 32};
+            be->launch_traceback(tp);
+            hp.ops = c->dOps.p;
+            hp.opsStart = c->dOpsStart.p;
+            hp.opsLen = c->dOpsLen.p;
+            hp.stage = HR_PATH_LEN;
+            hp.numItems = J;
+            be->launch_hit_res(hp);
+            done.push_back(std::move(c));
+        }
+        be->d2h(out->starts + lo, dStart.p, (size_t)span * sizeof(int));
+        stats.d2hBytes += 4LL * span;
+        if (!path) continue;
+        // every hit of the slice has its script length: one scan places them in hit order
+        be->launch_scan(dLen.p, span);
+        be->d2h(lenScan.data(), dLen.p, ((size_t)span + 1) * sizeof(int));
+        const int bytes = lenScan[(size_t)span];
+        DevBuf<uint8_t> dPool(be, (size_t)std::max(bytes, 1));
+        hp.pool = dPool.p;
+        hp.stage = HR_PATH_COPY;
+        for (auto& c : done) {
+            hp.nw = c->nw;
+            hp.numItems = c->jobs;
+            hp.jobHit = c->dJobHit.p;
+            hp.opsStride = c->opsStride;
+            hp.ops = c->dOps.p;
+            hp.opsStart = c->dOpsStart.p;
+            be->launch_hit_res(hp);
+        }
+        unsigned char* grown = static_cast<unsigned char*>(realloc(out->alignments, (size_t)std::max(poolAt + bytes, 1LL)));
+        if (!grown) throw std::runtime_error("out of memory for the hit alignments");
+        out->alignments = grown;
+        if (bytes) be->d2h(out->alignments + poolAt, dPool.p, (size_t)bytes);
+        for (int h = 0; h < span; ++h) out->alignmentOffsets[lo + h + 1] = poolAt + lenScan[(size_t)h + 1];
+        poolAt += bytes;
+        stats.d2hBytes += (long long)bytes + 4LL * (span + 1);
+    }
+    int err = 0;
+    dErr.download(&err, 1);
+    if (err) throw std::runtime_error("internal: a start-location / path sweep of a hit disagrees with its score");
+    trace.mark(path ? "hits: starts and paths" : "hits: starts");
 }
 }  // namespace eb

@@ -126,6 +126,37 @@ EDLIB_API int edlibB200FindHits(const char* const* queries, const int* queryLeng
 /* Frees the arrays of edlibB200FindHits and clears the struct. */
 EDLIB_API void edlibB200FreeHits(EdlibB200Hits* hits);
 
+/* The hits of edlibB200FindHits, with the start location and the alignment path of every stored hit.
+ *
+ * `hits` is exactly what edlibB200FindHits returns for the same arguments.  For a stored hit (c, s) of query q (rc(q)
+ * for a strand-1 hit) of m symbols, each hit taken on its own by the rules edlibAlign applies to its best hits:
+ *   start  (config.task EDLIB_TASK_LOC or EDLIB_TASK_PATH): the smallest st with ed(q, T[st..c]) = s, i.e. c minus the
+ *          last column of score s of the SHW alignment of rev(q) to rev(T[c-m-s+1..c]) (clipped at column 0);
+ *   script (EDLIB_TASK_PATH): the EDLIB_EDOP_* codes that edlibAlign(q, T[start..c], NW, k = -1, PATH) returns; its
+ *          cost is s.
+ * So the starts of the columns of a query's least score are edlibAlign(q, T, HW, k, LOC)'s startLocations, and the
+ * script of the first of them is edlibAlign(q, T, HW, k, PATH)'s alignment.  starts / scripts follow the stored hits
+ * in their order: starts[h] and alignments[alignmentOffsets[h] .. alignmentOffsets[h+1]) belong to hit h; a script
+ * turns into a CIGAR with edlibAlignmentToCigar.
+ *
+ * Accepted: everything edlibB200FindHits accepts, with config.task EDLIB_TASK_DISTANCE, EDLIB_TASK_LOC or
+ * EDLIB_TASK_PATH.  Anything else returns EDLIB_STATUS_ERROR with a message in edlibB200LastError (starting with
+ * "edlibB200FindHitAlignments:" for invalid input) and *out left empty; on success the arrays are malloc'd and
+ * edlibB200FreeHitAlignments releases them.  edlibB200LastStats reports what edlibB200FindHits reports; its kernel
+ * time and launch count include the start-location and path sweeps. */
+typedef struct {
+    EdlibB200Hits hits;           /* exactly what edlibB200FindHits returns for the same arguments */
+    int* starts;                  /* one per stored hit (task LOC / PATH), else NULL */
+    long long* alignmentOffsets;  /* task PATH: stored + 1 entries; hit h's script is alignments[off[h] .. off[h+1]) */
+    unsigned char* alignments;    /* EDLIB_EDOP_* codes, as EdlibAlignResult.alignment; NULL unless PATH */
+} EdlibB200HitAlignments;
+
+EDLIB_API int edlibB200FindHitAlignments(const char* const* queries, const int* queryLengths, int numQueries,
+                                         const char* target, int targetLength, const EdlibAlignConfig config,
+                                         int bothStrands, long long maxHitsPerQuery, EdlibB200HitAlignments* out);
+/* Frees the arrays of edlibB200FindHitAlignments and clears the struct. */
+EDLIB_API void edlibB200FreeHitAlignments(EdlibB200HitAlignments* out);
+
 /* A target kept resident on the device.  edlibAlignBatch calls of read sets (HW, short queries, plain equality) whose
  * targets[i] all equal (target, targetLength) of a live handle skip the target's upload, its encoding and the build of
  * its seed index: a caller that aligns many batches to one genome pays them once.  The bytes at `target` must not

@@ -2,6 +2,7 @@
 """Times edlibB200FindHits (all end locations within k) on the H100, next to the HW distance call on the same reads.
 
     python scripts/hits_probe.py [--reads 1000000] [--short 100000] [--repeats 3] [--out results.json]
+    python scripts/hits_probe.py --task loc|path [--reads 1000000] [--repeats 3] [--out results.json]
 
 Workloads: config-2 reads (150 bp, 3 % errors, seeded generator of bench.py) over the E. coli genome at k = 3 and 10
 (seed route) and, on fewer reads, k = 20 (above the largest seed threshold of a 150 bp read, 17: whole-target sweep);
@@ -9,7 +10,11 @@ seeded 23-mers at k = 4 (beyond every seed level's reach: whole-target sweep); a
 through edlibAlignBatch (HW distance).  Per workload: time per call (host clock around the whole call, median and
 spread over the repeats after one warm-up call), per-kernel device times of the last call (edlibB200LastKernelReport),
 hits per read, filterDecided / filterFallback.  The card's name and power limit are read in the same run.  Needs a
-GPU; prints one JSON document (and writes it to --out when given)."""
+GPU; prints one JSON document (and writes it to --out when given).
+
+--task loc / path times edlibB200FindHitAlignments instead (start locations / alignment paths of every hit) for the
+150 bp reads at k = 3 and 10, next to edlibB200FindHits of the same call (task DISTANCE) and edlibAlignBatch HW LOC /
+PATH of the same reads at the same k; the stored scripts' total length is reported for PATH."""
 import argparse
 import ctypes as C
 import json
@@ -22,7 +27,7 @@ REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO)
 
 from edlib_b200 import workloads  # noqa: E402
-from edlib_b200._ffi import AlignResult, Hits, make_config, product_path  # noqa: E402
+from edlib_b200._ffi import AlignResult, HitAlignments, Hits, make_config, product_path  # noqa: E402
 
 
 class Stats(C.Structure):  # include/edlib_b200.h EdlibB200Stats
@@ -33,7 +38,7 @@ class Stats(C.Structure):  # include/edlib_b200.h EdlibB200Stats
 
 def card():
     try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm,clocks.sm", "--format=csv,noheader"],
                              capture_output=True, text=True, timeout=60).stdout.strip()
     except Exception as e:  # noqa: BLE001
         out = "unknown (%s)" % e
@@ -46,6 +51,8 @@ def main():
     ap.add_argument("--reads-k20", type=int, default=10_000)  # k = 20 is above every seed level of 150 bp reads
     ap.add_argument("--short", type=int, default=100_000)
     ap.add_argument("--repeats", type=int, default=3)
+    ap.add_argument("--task", choices=("loc", "path"), default=None,
+                    help="time the start locations / paths of every hit instead of the hit lists")
     ap.add_argument("--out", default=None, help="also write the JSON document to this file")
     a = ap.parse_args()
     lib = C.CDLL(product_path())
@@ -55,6 +62,10 @@ def main():
     lib.edlibB200FindHits.argtypes = [C.POINTER(C.c_char_p), C.POINTER(C.c_int), C.c_int, C.c_char_p, C.c_int,
                                       type(make_config()[0]), C.c_int, C.c_longlong, C.POINTER(Hits)]
     lib.edlibB200FreeHits.argtypes = [C.POINTER(Hits)]
+    lib.edlibB200FindHitAlignments.restype = C.c_int
+    lib.edlibB200FindHitAlignments.argtypes = [C.POINTER(C.c_char_p), C.POINTER(C.c_int), C.c_int, C.c_char_p, C.c_int,
+                                               type(make_config()[0]), C.c_int, C.c_longlong, C.POINTER(HitAlignments)]
+    lib.edlibB200FreeHitAlignments.argtypes = [C.POINTER(HitAlignments)]
     lib.edlibAlignBatch.restype = C.c_int
     lib.edlibAlignBatch.argtypes = [C.POINTER(C.c_char_p), C.POINTER(C.c_int), C.POINTER(C.c_char_p), C.POINTER(C.c_int),
                                     C.c_int, type(make_config()[0]), C.POINTER(AlignResult)]
@@ -110,9 +121,30 @@ def main():
                  filterWindows=s.filterWindows, kernel_ms=round(s.kernelMs, 3), kernels=kern)
         return r
 
-    def distance_run(rs):
+    def alignments_run(rs, k, task):
         _, ptrs, lens, n = rs
-        cfg, _ = make_config(-1, 2, 0)
+        cfg, _ = make_config(k, 2, task)
+        info = {}
+
+        def call():
+            h = HitAlignments()
+            st = lib.edlibB200FindHitAlignments(ptrs, lens, n, tbuf, len(tbytes), cfg, 0, 1 << 40, C.byref(h))
+            assert st == 0
+            stored = h.hits.offsets[n]
+            info["hits"] = stored
+            info["script_bytes"] = h.alignmentOffsets[stored] if h.alignmentOffsets else 0
+            lib.edlibB200FreeHitAlignments(C.byref(h))
+        r = timed(call)
+        s, kern = last()
+        r.update(hits_per_read=round(info["hits"] / n, 3), filterDecided=s.filterDecided, filterFallback=s.filterFallback,
+                 kernel_ms=round(s.kernelMs, 3), kernels=kern)
+        if task == 2:
+            r["script_bytes"] = info["script_bytes"]
+        return r
+
+    def distance_run(rs, k=-1, task=0):
+        _, ptrs, lens, n = rs
+        cfg, _ = make_config(k, 2, task)
         tptr = (C.c_char_p * n)(*([C.cast(tbuf, C.c_char_p)] * n))
         tlen = (C.c_int * n)(*([len(tbytes)] * n))
         res = (AlignResult * n)()
@@ -125,6 +157,21 @@ def main():
         r.update(filterDecided=s.filterDecided, filterFallback=s.filterFallback, kernel_ms=round(s.kernelMs, 3), kernels=kern)
         return r
 
+    if a.task:
+        task = 1 if a.task == "loc" else 2
+        out = {"card": card(), "repeats": a.repeats, "warmup": 1, "reads": a.reads, "task": a.task}
+        long_reads = read_set(workloads.reads_of(genome, a.reads, read_len=150, seed=42))
+        for k in (3, 10):
+            out["hits_%s_150bp_k%d" % (a.task, k)] = alignments_run(long_reads, k, task)
+            out["hits_distance_150bp_k%d" % k] = hits_run(long_reads, k)
+            out["batch_%s_150bp_k%d" % (a.task, k)] = distance_run(long_reads, k, task)
+        out["card_after"] = card()
+        text = json.dumps(out, indent=1)
+        print(text)
+        if a.out:
+            with open(a.out, "w") as f:
+                f.write(text + "\n")
+        return
     out = {"card": card(), "repeats": a.repeats, "warmup": 1, "reads": a.reads, "reads_k20": a.reads_k20, "short_reads": a.short}
     long_reads = read_set(workloads.reads_of(genome, a.reads, read_len=150, seed=42))
     for k in (3, 10):
