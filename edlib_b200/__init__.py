@@ -126,27 +126,39 @@ def find_hits(queries, target, k, strands="forward", max_hits=None, additionalEq
     start whose alignment to [start, column] still has the hit's score).  task="path" adds "cigars" as well: the
     extended CIGAR of that alignment, as `align(..., task="path")` gives it; a "-" hit's CIGAR aligns the reverse
     complement.  For the columns of a query's least score these are exactly `align(query, target, "HW", task, k)`'s
-    locations, and its CIGAR is the one of the first of them."""
+    locations, and its CIGAR is the one of the first of them.
+
+    `target` given as a non-empty list or tuple of sequences (str, bytes, or lists / tuples of symbols; so a list of
+    single characters counts as records of one symbol) searches them as the records of one reference (chromosomes,
+    contigs) in one call.  The hits of a query on record r are exactly those of find_hits(query, target[r]): every hit
+    becomes (record, column, score) or (record, column, score, "+"/"-"), its column and "starts" count from the start
+    of its record, no hit spans two records, and hits are ordered by strand, then record, then column."""
     if strands not in ("forward", "both"):
         raise ValueError("strands must be 'forward' or 'both'")
     if task not in ("distance", "locations", "path"):
         raise ValueError("task must be 'distance', 'locations' or 'path'")
     queries = list(queries)
-    if strands == "both" and not all(_is_plain(s) for s in queries + [target]):
+    is_seq = lambda s: isinstance(s, (str, bytes, bytearray, list, tuple))  # noqa: E731
+    records = list(target) if isinstance(target, (list, tuple)) and target and all(map(is_seq, target)) else None
+    targets = records if records is not None else [target]
+    if strands == "both" and not all(_is_plain(s) for s in queries + targets):
         raise ValueError("strands='both' needs bytes or ASCII str sequences")
-    mapped, eqs = _map_to_bytes(queries + [target], additionalEqualities)
+    mapped, eqs = _map_to_bytes(queries + targets, additionalEqualities)
+    queries, targets = mapped[:len(queries)], mapped[len(queries):]
     both = strands == "both"
     cap = (1 << 62) if max_hits is None else max_hits
     lib = library()
-    if task == "distance":
-        st, res = lib.find_hits(mapped[:-1], mapped[-1], k, both, cap, eqs)
+    if records is not None:
+        st, res = lib.find_record_hits(queries, targets, k, both, cap, eqs, TASKS[task])
+    elif task == "distance":
+        st, res = lib.find_hits(queries, targets[0], k, both, cap, eqs)
     else:
-        st, res = lib.find_hit_alignments(mapped[:-1], mapped[-1], k, both, cap, eqs, TASKS[task])
+        st, res = lib.find_hit_alignments(queries, targets[0], k, both, cap, eqs, TASKS[task])
     if st != EDLIB_STATUS_OK:
         raise Exception("There was an error. (" + lib.lib.edlibB200LastError().decode() + ")")
     for r in res:
         if both:
-            r["hits"] = [(c, s, "-" if d else "+") for c, s, d in r["hits"]]
+            r["hits"] = [h[:-1] + ("-" if h[-1] else "+",) for h in r["hits"]]
         if "alignments" in r:
             r["cigars"] = [lib.cigar(a, EDLIB_CIGAR_EXTENDED) for a in r.pop("alignments")]
     return res

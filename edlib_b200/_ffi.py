@@ -44,8 +44,34 @@ class HitAlignments(C.Structure):         # include/edlib_b200.h EdlibB200HitAli
                 ("alignments", C.POINTER(C.c_ubyte))]
 
 
+class RecordHits(C.Structure):            # include/edlib_b200.h EdlibB200RecordHits (80 bytes)
+    _fields_ = [("aln", HitAlignments), ("records", C.POINTER(C.c_int))]
+
+
 assert C.sizeof(EqualityPair) == 2 and C.sizeof(AlignConfig) == 32 and C.sizeof(AlignResult) == 48
-assert C.sizeof(Hits) == 48 and C.sizeof(HitAlignments) == 72
+assert C.sizeof(Hits) == 48 and C.sizeof(HitAlignments) == 72 and C.sizeof(RecordHits) == 80
+
+
+def _hit_dicts(a, n, both, records):
+    """Per query of an EdlibB200HitAlignments: {"count", "hits"} and, when present, "starts" / "alignments"; hits are
+    (column, score[, strand]), prefixed by the record when `records` is given."""
+    h = a.hits
+    out = []
+    for i in range(n):
+        lo, hi = h.offsets[i], h.offsets[i + 1]
+        cols = [list(h.columns[lo:hi]), list(h.scores[lo:hi])]
+        if both:
+            cols.append(list(h.strands[lo:hi]))
+        if records is not None:
+            cols.insert(0, list(records[lo:hi]))
+        r = {"count": h.counts[i], "hits": list(zip(*cols))}
+        if a.starts:
+            r["starts"] = a.starts[lo:hi]
+        if a.alignments:
+            off, base = a.alignmentOffsets, C.cast(a.alignments, C.c_void_p).value
+            r["alignments"] = [C.string_at(base + off[j], off[j + 1] - off[j]) for j in range(lo, hi)]
+        out.append(r)
+    return out
 
 
 def make_config(k=-1, mode=EDLIB_MODE_NW, task=EDLIB_TASK_DISTANCE, equalities=None):
@@ -196,20 +222,33 @@ class EdlibLib:
         del keep
         if st != EDLIB_STATUS_OK:
             return st, None
-        h = a.hits
-        out = []
-        for i in range(n):
-            lo, hi = h.offsets[i], h.offsets[i + 1]
-            cols, scores = h.columns[lo:hi], h.scores[lo:hi]
-            r = {"count": h.counts[i],
-                 "hits": list(zip(cols, scores, h.strands[lo:hi])) if both else list(zip(cols, scores))}
-            if a.starts:
-                r["starts"] = a.starts[lo:hi]
-            if a.alignments:
-                off, base = a.alignmentOffsets, C.cast(a.alignments, C.c_void_p).value
-                r["alignments"] = [C.string_at(base + off[j], off[j + 1] - off[j]) for j in range(lo, hi)]
-            out.append(r)
+        out = _hit_dicts(a, n, both, None)
         self.lib.edlibB200FreeHitAlignments(C.byref(a))
+        return st, out
+
+    def find_record_hits(self, queries, records, k, both=False, max_hits=(1 << 62), equalities=None,
+                         task=EDLIB_TASK_DISTANCE, mode=EDLIB_MODE_HW):
+        """edlibB200FindRecordHits over a list of records.  Returns (status, [dict]) as find_hit_alignments, with
+        hits (record, column, score) or (record, column, score, strand); status != 0: (status, None)."""
+        fn = self.lib.edlibB200FindRecordHits
+        fn.restype = C.c_int
+        fn.argtypes = [C.POINTER(C.c_char_p), C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int),
+                       C.c_int, AlignConfig, C.c_int, C.c_longlong, C.POINTER(RecordHits)]
+        self.lib.edlibB200FreeRecordHits.restype = None
+        self.lib.edlibB200FreeRecordHits.argtypes = [C.POINTER(RecordHits)]
+        n, r = len(queries), len(records)
+        cfg, keep = make_config(k, mode, task, equalities)
+        qptr = (C.c_char_p * max(n, 1))(*queries)
+        qlen = (C.c_int * max(n, 1))(*[len(q) for q in queries])
+        rptr = (C.c_char_p * max(r, 1))(*records)
+        rlen = (C.c_int * max(r, 1))(*[len(x) for x in records])
+        a = RecordHits()
+        st = fn(qptr, qlen, n, rptr, rlen, r, cfg, 1 if both else 0, max_hits, C.byref(a))
+        del keep
+        if st != EDLIB_STATUS_OK:
+            return st, None
+        out = _hit_dicts(a.aln, n, both, a.records)
+        self.lib.edlibB200FreeRecordHits(C.byref(a))
         return st, out
 
     def _run_batch(self, call, queries, targets, k, mode, task, equalities):

@@ -463,15 +463,22 @@ EDLIB_API void edlibB200FreeCigars(char** cigars, int n) {
     eb::host_parallel_ranges((size_t)n, 16384, free_range);
 }
 
-// What edlibB200FindHits (alignments == false) / edlibB200FindHitAlignments refuse (include/edlib_b200.h), or "".
+// What edlibB200FindHits (alignments == false) / edlibB200FindHitAlignments / edlibB200FindRecordHits (records != NULL)
+// refuse (include/edlib_b200.h), or "".  Only lengths are read: a record's bytes are not touched here.
+struct RecordArgs {
+    const char* const* records;
+    const int* lengths;
+    int n;
+    int gap;  // separator symbols between two records (set here)
+};
 static std::string hits_input_error(const char* entry, bool alignments, const char* const* queries, const int* queryLengths,
-                                    int numQueries, const char* target, int targetLength, const EdlibAlignConfig& config,
-                                    int bothStrands, long long maxHits) {
+                                    int numQueries, const char* target, int targetLength, RecordArgs* records,
+                                    const EdlibAlignConfig& config, int bothStrands, long long maxHits) {
     const std::string at = std::string(entry) + ": ";
     if (numQueries < 0) return at + "numQueries < 0";
     if (numQueries > 0 && (!queries || !queryLengths)) return at + "no queries";
     if (bothStrands && numQueries > 0x3fffffff) return at + "too many queries for both strands";
-    if (!target || targetLength < 1) return at + "the target must have at least one symbol";
+    if (!records && (!target || targetLength < 1)) return at + "the target must have at least one symbol";
     if (config.mode != EDLIB_MODE_HW) return at + "mode must be EDLIB_MODE_HW";
     if (!alignments && config.task != EDLIB_TASK_DISTANCE) return at + "task must be EDLIB_TASK_DISTANCE";
     if (alignments && config.task != EDLIB_TASK_DISTANCE && config.task != EDLIB_TASK_LOC && config.task != EDLIB_TASK_PATH)
@@ -479,24 +486,41 @@ static std::string hits_input_error(const char* entry, bool alignments, const ch
     if (config.k < 0) return at + "k must be >= 0";
     if (maxHits < 0) return at + "maxHitsPerQuery must be >= 0";
     if (config.additionalEqualitiesLength > 0 && !config.additionalEqualities) return at + "no equality pairs";
-    for (int i = 0; i < numQueries; ++i)
+    int longest = 0;
+    for (int i = 0; i < numQueries; ++i) {
         if (!queries[i] || queryLengths[i] < 1 || queryLengths[i] > 256) return at + "query lengths must be 1 .. 256";
+        longest = std::max(longest, queryLengths[i]);
+    }
+    if (!records) return std::string();
+    if (records->n < 1) return at + "numRecords must be >= 1";
+    if (!records->records || !records->lengths) return at + "no records";
+    // an alignment that crosses a separator of gap symbols costs more than k and more than any query's length
+    records->gap = std::min(config.k, longest) + 1;
+    long long total = (long long)(records->n - 1) * records->gap;
+    for (int r = 0; r < records->n; ++r) {
+        if (!records->records[r] || records->lengths[r] < 1) return at + "every record must be non-NULL with at least one symbol";
+        total += records->lengths[r];
+    }
+    if (total > EDLIB_B200_MAX_RECORD_TARGET)
+        return at + "the records and their separators exceed EDLIB_B200_MAX_RECORD_TARGET symbols";
     return std::string();
 }
 
-// Both hit entries: `out` (never NULL here) is cleared, then filled on success; on failure nothing stays allocated.
+// The hit entries: `out` (never NULL here) is cleared, then filled on success; on failure nothing stays allocated.
+// records: a record call (edlibB200FindRecordHits), whose record of each stored hit goes to *recordsOut.
 static int find_hits_entry(const char* entry, bool alignments, bool outNull, const char* const* queries,
                            const int* queryLengths, int numQueries, const char* target, int targetLength,
-                           const EdlibAlignConfig& config, int bothStrands, long long maxHitsPerQuery,
-                           EdlibB200HitAlignments* out) {
+                           RecordArgs* records, const EdlibAlignConfig& config, int bothStrands, long long maxHitsPerQuery,
+                           EdlibB200HitAlignments* out, int** recordsOut) {
     std::lock_guard<std::mutex> lock(g_mu);
     eb::Engine* e = engine_locked();
     memset(out, 0, sizeof(*out));
+    if (recordsOut) *recordsOut = nullptr;
     if (!e) return EDLIB_STATUS_ERROR;  // no usable device: there is no CPU path
     t_lastEngine = e;
     const std::string bad = outNull ? std::string(entry) + (alignments ? ": out is NULL" : ": hits is NULL")
                                     : hits_input_error(entry, alignments, queries, queryLengths, numQueries, target,
-                                                       targetLength, config, bothStrands, maxHitsPerQuery);
+                                                       targetLength, records, config, bothStrands, maxHitsPerQuery);
     if (!bad.empty()) {
         e->lastError = bad;
         return EDLIB_STATUS_ERROR;
@@ -511,11 +535,22 @@ static int find_hits_entry(const char* entry, bool alignments, bool outNull, con
         e->lastError = "out of memory for the hit lists";
         return EDLIB_STATUS_ERROR;
     }
+    if (records) {  // one target laid out from the records: its length, no host pointer
+        targetLength = (records->n - 1) * records->gap;
+        for (int r = 0; r < records->n; ++r) targetLength += records->lengths[r];
+        target = nullptr;
+    }
     const std::vector<const char*> targets((size_t)numQueries, target);
     const std::vector<int> targetLengths((size_t)numQueries, targetLength);
     eb::BatchInput in{queries, queryLengths, targets.data(), targetLengths.data(), numQueries, config};
     in.strands = bothStrands != 0;
-    return e->find_hits(in, maxHitsPerQuery, out);
+    if (records) {
+        in.records = records->records;
+        in.recordLengths = records->lengths;
+        in.numRecords = records->n;
+        in.recordGap = records->gap;
+    }
+    return e->find_hits(in, maxHitsPerQuery, out, recordsOut);
 }
 
 EDLIB_API int edlibB200FindHits(const char* const* queries, const int* queryLengths, int numQueries, const char* target,
@@ -523,7 +558,7 @@ EDLIB_API int edlibB200FindHits(const char* const* queries, const int* queryLeng
                                 EdlibB200Hits* hits) {
     EdlibB200HitAlignments out;
     const int st = find_hits_entry("edlibB200FindHits", false, !hits, queries, queryLengths, numQueries, target,
-                                   targetLength, config, bothStrands, maxHitsPerQuery, &out);
+                                   targetLength, nullptr, config, bothStrands, maxHitsPerQuery, &out, nullptr);
     if (hits) *hits = out.hits;  // task DISTANCE: nothing else was allocated
     return st;
 }
@@ -537,11 +572,29 @@ EDLIB_API int edlibB200FindHitAlignments(const char* const* queries, const int* 
                                          int bothStrands, long long maxHitsPerQuery, EdlibB200HitAlignments* out) {
     EdlibB200HitAlignments scratch;
     return find_hits_entry("edlibB200FindHitAlignments", true, !out, queries, queryLengths, numQueries, target,
-                           targetLength, config, bothStrands, maxHitsPerQuery, out ? out : &scratch);
+                           targetLength, nullptr, config, bothStrands, maxHitsPerQuery, out ? out : &scratch, nullptr);
 }
 
 EDLIB_API void edlibB200FreeHitAlignments(EdlibB200HitAlignments* out) {
     if (out) eb::free_hit_alignments(out);
+}
+
+EDLIB_API int edlibB200FindRecordHits(const char* const* queries, const int* queryLengths, int numQueries,
+                                      const char* const* records, const int* recordLengths, int numRecords,
+                                      const EdlibAlignConfig config, int bothStrands, long long maxHitsPerQuery,
+                                      EdlibB200RecordHits* out) {
+    EdlibB200RecordHits scratch;
+    EdlibB200RecordHits* o = out ? out : &scratch;
+    RecordArgs ra{records, recordLengths, numRecords, 0};
+    return find_hits_entry("edlibB200FindRecordHits", true, !out, queries, queryLengths, numQueries, nullptr, 0, &ra,
+                           config, bothStrands, maxHitsPerQuery, &o->aln, &o->records);
+}
+
+EDLIB_API void edlibB200FreeRecordHits(EdlibB200RecordHits* out) {
+    if (!out) return;
+    eb::free_hit_alignments(&out->aln);
+    free(out->records);
+    out->records = nullptr;
 }
 
 EDLIB_API void edlibB200LastStats(EdlibB200Stats* s) {

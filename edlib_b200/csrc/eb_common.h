@@ -391,6 +391,8 @@ struct HitParams {
     const int* room;         // fill pass: [job] hits of the job that are stored (0: the job is skipped)
     int* cols;               // fill pass: end columns
     int* scores;             // fill pass: D(column)
+    const uint8_t* sepCodes; // record target (edlibB200FindRecordHits): its codes; a column holding code sep is a
+    int sep;                 // separator and never a hit (eb_core.h: RecordHitSink).  nullptr: one plain target
 };
 // Per read of a hits launch: the jobs of read `slot` are plan[slot].first .. + count (windows, in column order), or
 // slot + c * numReads for c < chunks (chunks, in column order).
@@ -444,6 +446,30 @@ struct HitResParams {
     int* len;                // [hits + 1] script length of each hit, then their exclusive prefix sums
     uint8_t* pool;           // dense scripts of the slice, in hit order
     int* err;                // set to 1 when a sweep disagrees with the score of its hit
+    const int* recOff;       // record target: [numRecords + 1] RecordParams::recOff (a start is clipped at the first
+    int numRecords;          // column of its hit's record); nullptr: one plain target
+};
+
+// Records of a multi-record target (edlibB200FindRecordHits): the records lie in order in one target, record r at
+// columns [recOff[r], recOff[r + 1] - gap), each followed by `gap` columns of the separator code sep (recOff[R] is the
+// target length + gap).  `stage` selects the per-item function of record_kernel.
+enum RecordStage : int {
+    REC_SEPARATORS = 0,  // item = target column c: tcodes[c] = sep when c is a separator column
+    REC_STARTS = 1,      // item = hit h of a slice: starts[h] -= first column of the record of stored hit firstHit + h
+    REC_HITS = 2,        // item = stored hit firstHit + h: records[.] = its record, cols[.] = its column in the record
+};
+struct RecordParams {
+    int stage;
+    int numItems;
+    const int* recOff;       // [numRecords + 1]
+    int numRecords;
+    int gap;
+    int sep;
+    uint8_t* tcodes;         // REC_SEPARATORS: the encoded target
+    long long firstHit;      // REC_STARTS / REC_HITS: stored slot of item 0
+    int* cols;               // [stored hit] end column in the target (REC_HITS: in its record, afterwards)
+    int* starts;             // REC_STARTS: [item] start of the hit in the target -> in its record
+    int* records;            // REC_HITS: [stored hit] record
 };
 
 // ---------------------------------------------------------------------------------------------

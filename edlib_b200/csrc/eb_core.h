@@ -386,11 +386,29 @@ EB_HD bool hit_sink_open(const HitParams& h, int job, HitSink& s) {
     s.scores = h.at ? h.scores + h.at[job] : nullptr;
     return !h.at || s.room > 0;
 }
+// The sink of a record target (HitParams::sepCodes): a separator column is never a hit, so the count pass sees exact
+// counts.  Its own kernel instances run it; the plain sink stays free of the test.
+struct RecordHitSink : HitSink {
+    const uint8_t* sepCodes;
+    int sep;
+    EB_HD void hit(int score, int column) {
+        if (sepCodes[column] != sep) HitSink::hit(score, column);
+    }
+};
+EB_HD bool hit_sink_open(const HitParams& h, int job, RecordHitSink& s) {
+    s.sepCodes = h.sepCodes;
+    s.sep = h.sep;
+    return hit_sink_open(h, job, static_cast<HitSink&>(s));
+}
 EB_HD void hit_sink_close(const HitParams& h, int job, const HitSink& s) {
     if (!h.at) h.count[job] = s.count;
 }
 template <int NW, bool RANGE = false>
 EB_HD void k1_event(K1State<NW>&, int score, int column, HitSink* sink, int, Ovf*, int*, int) {
+    sink->hit(score, column);
+}
+template <int NW, bool RANGE = false>
+EB_HD void k1_event(K1State<NW>&, int score, int column, RecordHitSink* sink, int, Ovf*, int*, int) {
     sink->hit(score, column);
 }
 
@@ -649,7 +667,7 @@ struct K1Band {
             const uint64_t M = kb >= 63 ? 0ull : (~0ull << (kb + 1));
             const int score = S - popcount32(VP0 & (uint32_t)M) - popcount32(VP1 & (uint32_t)(M >> 32)) +
                               popcount32(VN0 & (uint32_t)M) + popcount32(VN1 & (uint32_t)(M >> 32));
-            if constexpr (std::is_same<RecT, HitSink>::value) {
+            if constexpr (std::is_base_of<HitSink, RecT>::value) {
                 if (score <= best) rec->hit(score, ws + j);  // hits: best is the fixed threshold
             } else if (score <= best) {  // same bookkeeping as k1_event (ref cpp:658-673)
                 constexpr int CAP = (int)(sizeof(rec->pos) / sizeof(rec->pos[0]));
@@ -782,9 +800,9 @@ EB_HD void k1w_thread(const K1WParams& p, int slot, WAcc& acc) {
 // held fixed; every tracked column scoring <= t is a hit.  The tracked columns of a read's windows cover every end
 // column of every alignment within t, and every such score is exact (seed_windows), so the hits of a read are those of
 // its windows in window order.  The early exits stay valid: they only leave windows that hold no score <= t.
-template <int NW, class WAcc>
+template <int NW, class WAcc, class Sink = HitSink>
 EB_HD void k1w_hits_thread(const K1WParams& p, const HitParams& h, int slot, WAcc& acc) {
-    HitSink sink;
+    Sink sink;
     if (!hit_sink_open(h, slot, sink)) return;
     const int pair = p.readList[slot];
     const int m = p.qlen[pair];
@@ -817,10 +835,10 @@ EB_HD void k1w_hits_thread(const K1WParams& p, const HitParams& h, int slot, WAc
 
 // Hits of one (chunk, read) job of a whole-target HW sweep (K1Params chunk geometry, kInit = k): the chunk restarts
 // halo >= 2m columns early, so every score of the columns it owns is exact, and it reports only those.
-template <int NW, class Acc>
+template <int NW, class Acc, class Sink = HitSink>
 EB_HD void k1_hits_thread(const K1Params& p, const HitParams& h, int slot, int chunk, Acc& acc) {
     const int job = chunk * p.numReads + slot;
-    HitSink sink;
+    Sink sink;
     if (!hit_sink_open(h, job, sink)) return;
     const int pair = p.readList[slot];
     const int m = p.qlen[pair];
@@ -871,16 +889,24 @@ EB_HD void hits_place_item(const HitPlaceParams& p, int slot) {
 // =============================================================================================
 
 // Radix key of the Lidx codes at s (eb_common.h: SeedIndexParams); only `avail` codes exist, the rest count as 0.
+// SEP (a record target): a code >= sigma is a separator and counts as 0 too, so that a seed that ends right before a
+// separator is still found by the range lookup of its shorter key.
+template <bool SEP = false>
 EB_HD uint32_t seed_key(const uint8_t* s, int avail, int Lidx, uint32_t sigma) {
     uint32_t key = 0;
-    for (int x = 0; x < Lidx; ++x) key = key * sigma + (x < avail ? (uint32_t)s[x] : 0u);
+    for (int x = 0; x < Lidx; ++x) {
+        const uint32_t c = x < avail ? (uint32_t)s[x] : 0u;
+        key = key * sigma + ((SEP && c >= sigma) ? 0u : c);
+    }
     return key;
 }
+template <bool SEP = false>
 EB_HD void seed_count_item(const SeedIndexParams& p, int i) {
-    atomic_add_int(p.bucketStart + seed_key(p.tcodes + i, p.n - i, p.Lidx, (uint32_t)p.sigma), 1);
+    atomic_add_int(p.bucketStart + seed_key<SEP>(p.tcodes + i, p.n - i, p.Lidx, (uint32_t)p.sigma), 1);
 }
+template <bool SEP = false>
 EB_HD void seed_fill_item(const SeedIndexParams& p, int i) {
-    const uint32_t b = seed_key(p.tcodes + i, p.n - i, p.Lidx, (uint32_t)p.sigma);
+    const uint32_t b = seed_key<SEP>(p.tcodes + i, p.n - i, p.Lidx, (uint32_t)p.sigma);
     p.positions[p.bucketStart[b] + atomic_add_int(p.cursor + b, 1)] = i;
 }
 
@@ -1521,6 +1547,17 @@ EB_HD int hit_res_pair(const HitResParams& p, long long slot) {  // last pair wh
     return lo;
 }
 
+// Record of target column c of a record target (eb_common.h: RecordParams): the last r with recOff[r] <= c.
+EB_HD int record_of(const int* recOff, int numRecords, int c) {
+    int lo = 0, hi = numRecords - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (recOff[mid] <= c) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+
 EB_HD void hit_res_item(const HitResParams& p, int i) {
     switch (p.stage) {
         case HR_FLAG: {
@@ -1540,7 +1577,8 @@ EB_HD void hit_res_item(const HitResParams& p, int i) {
             J.matOff = 0;
             J.m = m;
             const long long span = (long long)m + s;  // a start further back costs more than s
-            J.n = (int)((long long)c + 1 < span ? (long long)c + 1 : span);
+            const int first = p.recOff ? p.recOff[record_of(p.recOff, p.numRecords, c)] : 0;  // nor before the record
+            J.n = (int)((long long)c - first + 1 < span ? (long long)c - first + 1 : span);
             J.kInit = s + 1;
             J.trackFrom = 0;
             p.jobs[j] = J;
@@ -1601,6 +1639,30 @@ EB_HD void hit_res_item(const HitResParams& p, int i) {
             const uint8_t* src = p.ops + (uint64_t)i * p.opsStride + (uint64_t)p.opsStart[i];
             uint8_t* dst = p.pool + p.len[h];
             for (int x = 0; x < len; ++x) dst[x] = src[x];
+            break;
+        }
+        default: break;
+    }
+}
+
+// One item of record_kernel (eb_common.h: RecordParams).
+EB_HD void record_item(const RecordParams& p, int i) {
+    switch (p.stage) {
+        case REC_SEPARATORS: {
+            const int r = record_of(p.recOff, p.numRecords, i);
+            if (i >= p.recOff[r + 1] - p.gap) p.tcodes[i] = (uint8_t)p.sep;
+            break;
+        }
+        case REC_STARTS: {
+            const int c = p.cols[p.firstHit + i];
+            p.starts[i] -= p.recOff[record_of(p.recOff, p.numRecords, c)];
+            break;
+        }
+        case REC_HITS: {
+            const long long h = p.firstHit + i;
+            const int r = record_of(p.recOff, p.numRecords, p.cols[h]);
+            p.records[h] = r;
+            p.cols[h] -= p.recOff[r];
             break;
         }
         default: break;

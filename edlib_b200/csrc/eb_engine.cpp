@@ -166,6 +166,10 @@ Prepared* Engine::take_prepared(const BatchInput& in) {
     p->tg.clear();
     p->hasEq = false;
     p->ncodes = 0;
+    p->recOff.clear();
+    p->dRecOff.reset();
+    p->recGap = 0;
+    p->sep = -1;
     p->computed = false;
     p->classified = false;
     p->groups.clear();
@@ -268,6 +272,15 @@ Prepared* Engine::prepare(const BatchInput& in) {
         }
         const int T = (int)p->tg.size();
         trace.mark("prepare: lengths + distinct targets");
+        // a record target: record r at columns recOff[r] .., then recGap separator columns (eb_common.h: RecordParams)
+        const int numRec = in.numRecords;
+        if (numRec > 0) {
+            if (T != 1) throw std::runtime_error("internal: a record target is the one target of its batch");
+            p->recGap = in.recordGap;
+            p->recOff.assign((size_t)numRec + 1, 0);
+            for (int r = 0; r < numRec; ++r) p->recOff[(size_t)r + 1] = p->recOff[(size_t)r] + in.recordLengths[r] + in.recordGap;
+            if (p->recOff[(size_t)numRec] - in.recordGap != p->tg[0].len) throw std::runtime_error("internal: record target length");
+        }
 
         // pack: queries back to back, then every target 16-aligned with >= 16 bytes of slack
         size_t total = 0;
@@ -317,6 +330,12 @@ Prepared* Engine::prepare(const BatchInput& in) {
             auto copy_item = [&](int it) {
                 if (it < N) {
                     if (p->qlen[it]) memcpy(stage + p->qoff[it], in.queries[it], (size_t)p->qlen[it]);
+                } else if (numRec > 0) {  // the records, zeros in the separators until they are written after the encoding
+                    uint8_t* dst = stage + p->tg[0].off;
+                    for (int r = 0; r < numRec; ++r) {
+                        memcpy(dst + p->recOff[(size_t)r], in.records[r], (size_t)in.recordLengths[r]);
+                        if (r + 1 < numRec) memset(dst + p->recOff[(size_t)r + 1] - p->recGap, 0, (size_t)p->recGap);
+                    }
                 } else {
                     const Target& g = p->tg[it - N];
                     if (g.len) memcpy(stage + g.off, g.ptr, (size_t)g.len);
@@ -404,7 +423,11 @@ Prepared* Engine::prepare(const BatchInput& in) {
             for (int s0 = 0; s0 < len; s0 += 65536) items.push_back(MaskItem{off + (uint64_t)s0, std::min(65536, len - s0), dst});
         };
         for (int i : longQueries) add_items(p->qoff[i], p->qlen[i], i);
-        for (int t = 0; t < T; ++t) add_items(p->tg[t].off, p->tg[t].len, N + t);
+        if (numRec > 0) {  // the records only: no separator byte enters a presence set
+            for (int r = 0; r < numRec; ++r) add_items(p->tg[0].off + (uint64_t)p->recOff[(size_t)r], in.recordLengths[r], N);
+        } else {
+            for (int t = 0; t < T; ++t) add_items(p->tg[t].off, p->tg[t].len, N + t);
+        }
         HostBuf<int> tset(be, (size_t)N);
         parallel_ranges((size_t)N, 65536, [&](size_t lo, size_t hi) {
             for (size_t i = lo; i < hi; ++i) tset[i] = N + p->tidx[i];
@@ -504,10 +527,41 @@ Prepared* Engine::prepare(const BatchInput& in) {
                 anyEq = false;  // nothing left for the table
             }
         }
+        // more than one record: the separator takes the code after the batch's codes; it matches nothing, not even a
+        // wildcard (its row and column of the equality table stay 0)
+        if (numRec > 1) {
+            if (p->ncodes >= 256)
+                throw std::runtime_error("edlibB200FindRecordHits: the queries and records use all 256 codes: none is left for "
+                                         "the separator between records");
+            p->sep = p->ncodes++;
+            if (anyEq) {
+                const int s0 = p->sep, s1 = p->ncodes;
+                std::vector<uint8_t> grown((size_t)s1 * s1, 0);
+                for (int a = 0; a < s0; ++a)
+                    for (int b = 0; b < s0; ++b) grown[(size_t)a * s1 + b] = eq[(size_t)a * s0 + b];
+                eq.swap(grown);
+            }
+        }
         DevBuf<uint8_t> dMap(be, 256);
         dMap.upload(map, 256);
         EncodeParams ep{p->dSeq.p, (uint64_t)devTotal, dMap.p};
         be->launch_encode(ep);
+        if (numRec > 0) {
+            p->dRecOff.alloc(be, (size_t)numRec + 1);
+            p->dRecOff.upload(p->recOff.data(), (size_t)numRec + 1);
+        }
+        if (numRec > 1) {  // separator columns: written over the encoded zeros, before any sweep or index build reads them
+            RecordParams rp;
+            memset(&rp, 0, sizeof(rp));
+            rp.stage = REC_SEPARATORS;
+            rp.numItems = p->tg[0].len;
+            rp.recOff = p->dRecOff.p;
+            rp.numRecords = numRec;
+            rp.gap = p->recGap;
+            rp.sep = p->sep;
+            rp.tcodes = p->dSeq.p + p->tg[0].off;
+            be->launch_record(rp);
+        }
         if (anyEq) {
             p->dEqtab.alloc(be, eq.size());
             p->dEqtab.upload(eq.data(), eq.size());
@@ -823,6 +877,7 @@ void Engine::release(Prepared* p) {
     p->dQoff.reset();
     p->dQlen.reset();
     p->dEqtab.reset();
+    p->dRecOff.reset();
     p->computed = false;
     if (spare_) {
         delete p;
@@ -927,11 +982,12 @@ void free_hit_alignments(EdlibB200HitAlignments* h) {
 
 // The grouped batch of every query against the one target (a strand batch for both strands), then the hits pass
 // instead of the distance pass.
-int Engine::find_hits(const BatchInput& in, long long maxHits, EdlibB200HitAlignments* out) {
+int Engine::find_hits(const BatchInput& in, long long maxHits, EdlibB200HitAlignments* out, int** records) {
     Prepared* p = nullptr;
     stats = EngineStats();
     statsPending_ = false;
     memset(out, 0, sizeof(*out));
+    if (records) *records = nullptr;
     try {
         BatchInput din = in;  // the batch itself is that of edlibB200FindHits: the task only adds a stage
         din.config.task = EDLIB_TASK_DISTANCE;
@@ -939,7 +995,7 @@ int Engine::find_hits(const BatchInput& in, long long maxHits, EdlibB200HitAlign
         be_->reset_timing();
         {
             Pass ps(*this, be_, p);
-            ps.hits(maxHits, in.config.task, out);
+            ps.hits(maxHits, in.config.task, out, records);
         }
         be_->sync_all();
         be_->release_marks();
@@ -952,6 +1008,10 @@ int Engine::find_hits(const BatchInput& in, long long maxHits, EdlibB200HitAlign
         quiesce();
         if (p) release(p);
         free_hit_alignments(out);
+        if (records) {
+            free(*records);
+            *records = nullptr;
+        }
         return EDLIB_STATUS_ERROR;
     }
 }

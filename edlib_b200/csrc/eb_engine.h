@@ -93,6 +93,11 @@ struct Backend {
     virtual void launch_hits_place(const HitPlaceParams&) { no_kernel("hits_place"); }
     // start locations / edit scripts of stored hits (eb_common.h: HitResParams)
     virtual void launch_hit_res(const HitResParams&) { no_kernel("hit_res"); }
+    // records of a multi-record target (eb_common.h: RecordParams), and the seed index of such a target, whose keys
+    // read the separator code as 0 (launch_seed_count / launch_seed_fill otherwise)
+    virtual void launch_record(const RecordParams&) { no_kernel("record"); }
+    virtual void launch_seed_count_records(const SeedIndexParams&) { no_kernel("seed_count_records"); }
+    virtual void launch_seed_fill_records(const SeedIndexParams&) { no_kernel("seed_fill_records"); }
     [[noreturn]] static void no_kernel(const char* name) {
         throw std::runtime_error(std::string(name) + ": no such kernel on this backend");
     }
@@ -111,6 +116,12 @@ struct BatchInput {
     int numPairs;
     EdlibAlignConfig config;
     bool strands = false;  // align every query and its reverse complement, report the better strand (Prepared::strands)
+    // A record target (edlibB200FindRecordHits; targets[i] == nullptr, targetLengths[i] == the laid-out length): the
+    // records in order, each but the last followed by recordGap separator columns.  numRecords == 0: plain targets.
+    const char* const* records = nullptr;
+    const int* recordLengths = nullptr;
+    int numRecords = 0;
+    int recordGap = 0;
 };
 
 struct EngineTunables {
@@ -199,8 +210,10 @@ public:
     // edlibB200FindHits / edlibB200FindHitAlignments: every end column within config.k of every query over the one
     // shared target (in.strands: of its reverse complement too), at most maxHits stored per query; config.task LOC /
     // PATH adds the start location / edit script of every stored hit.  `out` is filled with malloc'd arrays; on
-    // failure nothing stays allocated.  Returns EDLIB_STATUS_OK / EDLIB_STATUS_ERROR.
-    int find_hits(const BatchInput& in, long long maxHits, EdlibB200HitAlignments* out);
+    // failure nothing stays allocated.  Returns EDLIB_STATUS_OK / EDLIB_STATUS_ERROR.  A record target
+    // (in.numRecords > 0, edlibB200FindRecordHits): columns and starts count from the start of each hit's record, and
+    // *records receives the record of every stored hit (malloc'd).
+    int find_hits(const BatchInput& in, long long maxHits, EdlibB200HitAlignments* out, int** records = nullptr);
 
     void finish_stats();  // fills the device-time fields of `stats` for the last pass (on demand)
 

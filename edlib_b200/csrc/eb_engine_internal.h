@@ -372,6 +372,13 @@ public:
     bool hasEq = false;
     int ncodes = 0;
     PinnedVec<int> alphaLen;
+    // A record target (BatchInput::numRecords > 0): tg[0] holds the records, recOff the first column of each
+    // (eb_common.h: RecordParams; numRecords + 1 entries) on the host and the device.  With more than one record, the
+    // separator code sep = ncodes - 1 matches nothing; sep == -1: no separator.
+    std::vector<int> recOff;
+    DevBuf<int> dRecOff;
+    int recGap = 0;
+    int sep = -1;
 
     // classification (Engine::classify): pairs per (target, word class) for the lane kernels, the rest
     struct Part {
@@ -471,7 +478,9 @@ struct SeedIndex {
 };
 
 // Builds the radix seed index of an encoded target (seed lengths per level, bucket table, positions).
-bool build_seed_index(Backend* be, const EngineTunables& tun, SeedIndex& sx, const uint8_t* tcodes, int n, int ncodes);
+// separators: a record target whose separator code (>= ncodes) is left out of the radix (keys read it as 0)
+bool build_seed_index(Backend* be, const EngineTunables& tun, SeedIndex& sx, const uint8_t* tcodes, int n, int ncodes,
+                      bool separators = false);
 
 // The codes of a target encoded by its own alphabet (encode_target, eb_engine.cpp): dense codes of its bytes in ascending
 // order, every byte it lacks one extra code that matches nothing.
@@ -724,7 +733,8 @@ struct Pass {
     // seed windows of the first level whose threshold reaches k, or the whole-target sweep (no such level, saturated
     // plan, repeats, short target, equality table); both count, place, then fill.  task LOC / PATH: then the start
     // location / edit script of every stored hit (hit_alignments).
-    void hits(long long maxHits, int task, EdlibB200HitAlignments* out);
+    // A record target: columns (and starts) are mapped into their records on the device, their records into *records.
+    void hits(long long maxHits, int task, EdlibB200HitAlignments* out, int** records);
     // Start locations (and, task PATH, edit scripts) of the S stored hits in dCols / dScores, whose pairs start at
     // dBase: lane sweeps per word class over slices of stored hits, jobs built on the device (eb_core.h: hit_res_item).
     void hit_alignments(int task, long long S, const std::vector<long long>& stored, const long long* dBase,

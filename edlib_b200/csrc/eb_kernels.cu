@@ -337,6 +337,17 @@ __global__ void __launch_bounds__(THREADS) k1w_hits_kernel(const K1WParams p, co
     k1w_hits_thread<NW>(p, h, slot, acc);
 }
 
+// The same over a record target: separator columns are no hits (eb_core.h: RecordHitSink).
+template <int NW, int THREADS>
+__global__ void __launch_bounds__(THREADS) k1w_hits_records_kernel(const K1WParams p, const HitParams h) {
+    extern __shared__ __align__(128) unsigned char smem[];
+    const int slot = blockIdx.x * THREADS + threadIdx.x;
+    if (slot >= p.numReads) return;
+    SmemWordAcc<THREADS, NW + 4> acc;
+    acc.base = smem_u32(smem) + 4u * threadIdx.x;
+    k1w_hits_thread<NW, SmemWordAcc<THREADS, NW + 4>, RecordHitSink>(p, h, slot, acc);
+}
+
 // Hits of a whole-target sweep (eb_core.h: k1_hits_thread): one thread per (read, chunk), symbols from global memory
 // (L2), the profile in shared memory as for lane_kernel.
 template <int NW>
@@ -350,6 +361,17 @@ __global__ void k1_hits_kernel(const K1Params p, const HitParams h) {
     acc.b0 = smem_u32(smem) + 16u * blockDim.x + 4u * SmemPeqAcc<NW>::NWB * threadIdx.x;
     k1_hits_thread<NW>(p, h, slot, (int)blockIdx.y, acc);
 }
+template <int NW>
+__global__ void k1_hits_records_kernel(const K1Params p, const HitParams h) {
+    extern __shared__ __align__(128) unsigned char smem[];
+    const int slot = blockIdx.x * blockDim.x + threadIdx.x;
+    if (slot >= p.numReads) return;
+    SmemPeqAcc<NW> acc;
+    acc.codeStride = (uint32_t)blockDim.x * (16u + 4u * SmemPeqAcc<NW>::NWB);
+    acc.a0 = smem_u32(smem) + 16u * threadIdx.x;
+    acc.b0 = smem_u32(smem) + 16u * blockDim.x + 4u * SmemPeqAcc<NW>::NWB * threadIdx.x;
+    k1_hits_thread<NW, SmemPeqAcc<NW>, RecordHitSink>(p, h, slot, (int)blockIdx.y, acc);
+}
 
 __global__ void hits_total_kernel(const HitPlaceParams p) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -362,6 +384,10 @@ __global__ void hits_place_kernel(const HitPlaceParams p) {
 __global__ void hit_res_kernel(const HitResParams p) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < p.numItems) hit_res_item(p, i);
+}
+__global__ void record_kernel(const RecordParams p) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < p.numItems) record_item(p, i);
 }
 
 // L: one alignment per thread over its own target (eb_core.h: lane_job).
@@ -453,6 +479,15 @@ __global__ void seed_count_kernel(const SeedIndexParams p) {
 __global__ void seed_fill_kernel(const SeedIndexParams p) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < p.numPos) seed_fill_item(p, i);
+}
+// the index of a record target: separator codes (>= sigma) count as 0 in the keys
+__global__ void seed_count_records_kernel(const SeedIndexParams p) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < p.numPos) seed_count_item<true>(p, i);
+}
+__global__ void seed_fill_records_kernel(const SeedIndexParams p) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < p.numPos) seed_fill_item<true>(p, i);
 }
 // One read per group of GW lanes (16: two reads per warp; 32: a warp per read).  The lanes take the seeds of the
 // read, so their index lookups (key -> bucket bounds -> positions -> target symbols, a chain of dependent random
@@ -986,7 +1021,9 @@ struct CudaBackend : Backend {
         with_nw(nw, [&](auto w) {
             with_one_of<128, 64, 32>(block, "bad K1W CTA size", [&](auto threads) {
                 constexpr int THREADS = decltype(threads)::value;
-                launch("k1w_hits", k1w_hits_kernel<decltype(w)::value, THREADS>, (p.numReads + THREADS - 1) / THREADS, THREADS, smem, p, h);
+                const int blocks = (p.numReads + THREADS - 1) / THREADS;
+                if (h.sepCodes) launch("k1w_hits_records", k1w_hits_records_kernel<decltype(w)::value, THREADS>, blocks, THREADS, smem, p, h);
+                else launch("k1w_hits", k1w_hits_kernel<decltype(w)::value, THREADS>, blocks, THREADS, smem, p, h);
             });
         });
     }
@@ -998,7 +1035,10 @@ struct CudaBackend : Backend {
         const size_t smem = perThread * block;
         if (smem > (size_t)maxSmemOptin) throw std::runtime_error("K1: alphabet too large for shared memory");
         const dim3 grid((p.numReads + block - 1) / block, p.chunks);
-        with_nw(nw, [&](auto w) { launch("k1_hits", k1_hits_kernel<decltype(w)::value>, grid, block, smem, p, h); });
+        with_nw(nw, [&](auto w) {
+            if (h.sepCodes) launch("k1_hits_records", k1_hits_records_kernel<decltype(w)::value>, grid, block, smem, p, h);
+            else launch("k1_hits", k1_hits_kernel<decltype(w)::value>, grid, block, smem, p, h);
+        });
     }
     void launch_hits_total(const HitPlaceParams& p) override {
         if (p.numReads > 0) launch("hits_total", hits_total_kernel, (p.numReads + 255) / 256, 256, 0, p);
@@ -1008,6 +1048,9 @@ struct CudaBackend : Backend {
     }
     void launch_hit_res(const HitResParams& p) override {
         if (p.numItems > 0) launch("hit_res", hit_res_kernel, (p.numItems + 255) / 256, 256, 0, p);
+    }
+    void launch_record(const RecordParams& p) override {
+        if (p.numItems > 0) launch("record", record_kernel, (p.numItems + 255) / 256, 256, 0, p);
     }
     void launch_lane(const LParams& p, int nw, int mode, bool rev, bool store) override {
         int block = 128;
@@ -1046,6 +1089,12 @@ struct CudaBackend : Backend {
     }
     void launch_seed_count(const SeedIndexParams& p) override { launch("seed_count", seed_count_kernel, (p.numPos + 255) / 256, 256, 0, p); }
     void launch_seed_fill(const SeedIndexParams& p) override { launch("seed_fill", seed_fill_kernel, (p.numPos + 255) / 256, 256, 0, p); }
+    void launch_seed_count_records(const SeedIndexParams& p) override {
+        launch("seed_count_records", seed_count_records_kernel, (p.numPos + 255) / 256, 256, 0, p);
+    }
+    void launch_seed_fill_records(const SeedIndexParams& p) override {
+        launch("seed_fill_records", seed_fill_records_kernel, (p.numPos + 255) / 256, 256, 0, p);
+    }
     void launch_scan(int* data, int count) override {
         if (count <= 0) {  // no tiles (a launch of no CTAs is refused): only the total, 0
             zero(data, sizeof(int));

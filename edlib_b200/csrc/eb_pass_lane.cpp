@@ -10,7 +10,8 @@ namespace eb {
 // sweep); the later levels shorter ones (more seeds fit into a read, so a higher threshold, at the price of more
 // chance occurrences) for the reads the previous level could not decide.  One table with keys of Lidx symbols
 // (sigma^Lidx <= 2n buckets) serves all of them.
-bool build_seed_index(Backend* be, const EngineTunables& tun, SeedIndex& sx, const uint8_t* tcodes, int n, int ncodes) {
+bool build_seed_index(Backend* be, const EngineTunables& tun, SeedIndex& sx, const uint8_t* tcodes, int n, int ncodes,
+                      bool separators) {
     sx.n = n;
     sx.ok = false;
     const int sigma = std::max(2, ncodes);
@@ -56,9 +57,11 @@ bool build_seed_index(Backend* be, const EngineTunables& tun, SeedIndex& sx, con
     ip.bucketStart = sx.bucketStart.p;
     ip.cursor = cursor.p;
     ip.positions = sx.positions.p;
-    be->launch_seed_count(ip);
+    if (separators) be->launch_seed_count_records(ip);
+    else be->launch_seed_count(ip);
     be->launch_scan(sx.bucketStart.p, (int)keys);
-    be->launch_seed_fill(ip);
+    if (separators) be->launch_seed_fill_records(ip);
+    else be->launch_seed_fill(ip);
     sx.ok = true;
     return true;
 }
@@ -70,7 +73,8 @@ bool Pass::seed_index(int t) {
     const int n = tg.len;
     if (sx.target == t && sx.n == n) return sx.ok;
     sx.target = t;
-    const bool ok = build_seed_index(be, tun, sx, p->dSeq.p + tg.off, n, p->ncodes);
+    // a record target: the radix is that of the records' codes, without the separator
+    const bool ok = build_seed_index(be, tun, sx, p->dSeq.p + tg.off, n, p->sep >= 0 ? p->sep : p->ncodes, p->sep >= 0);
     trace.mark("filter: seed index");
     return ok;
 }
@@ -956,11 +960,13 @@ struct HitRun {
 constexpr int HIT_RUN_READS = 1 << 18;  // reads per launch group (bounds the per-job arrays of a whole-target sweep)
 }  // namespace
 
-void Pass::hits(long long maxHits, int task, EdlibB200HitAlignments* outAln) {
+void Pass::hits(long long maxHits, int task, EdlibB200HitAlignments* outAln, int** records) {
     EdlibB200Hits* out = &outAln->hits;
     if (p->tg.size() != 1) throw std::runtime_error("internal: hits need one shared target");
     const Target& tg = p->tg[0];
     const int n = tg.len;
+    // several records: the sweeps run over all of them at once, and a separator column is never a hit
+    const uint8_t* sepCodes = p->sep >= 0 ? p->dSeq.p + tg.off : nullptr;
     const int Q = p->strands ? N / 2 : N;
     // ---- routes: the first seed level whose threshold reaches k itself, else the whole-target sweep ----
     const bool seeds = n >= tun.filterMinTarget && !p->hasEq && tun.filterSeedK > 0 && tun.filterSeedLevels > 0 && seed_index(0);
@@ -1019,7 +1025,7 @@ void Pass::hits(long long maxHits, int task, EdlibB200HitAlignments* outAln) {
         }
         r.dCount.alloc(be, (size_t)std::max(r.numJobs, 1));
         if (r.numJobs > 0) {
-            const HitParams h{r.dCount.p, nullptr, nullptr, nullptr, nullptr};
+            const HitParams h{r.dCount.p, nullptr, nullptr, nullptr, nullptr, sepCodes, p->sep};
             be->launch_k1w_hits(window_params(tg, r.jobs, r.numJobs), h, r.nw);
         }
         HitPlaceParams hp;
@@ -1067,7 +1073,7 @@ void Pass::hits(long long maxHits, int task, EdlibB200HitAlignments* outAln) {
             kp.chunks = r.chunks;
             kp.chunkLen = r.chunkLen;
             kp.halo = 64 * nw;
-            const HitParams h{r.dCount.p, nullptr, nullptr, nullptr, nullptr};
+            const HitParams h{r.dCount.p, nullptr, nullptr, nullptr, nullptr, sepCodes, p->sep};
             be->launch_k1_hits(kp, h, nw);
             stats.k1Cells += (long long)g * 32 * nw * (long long)n;
             HitPlaceParams hp;
@@ -1111,6 +1117,11 @@ void Pass::hits(long long maxHits, int task, EdlibB200HitAlignments* outAln) {
     if (!out->columns || !out->scores || (p->strands && !out->strands)) throw std::runtime_error("out of memory for the hit lists");
     if (p->strands)
         for (int pair = 0; pair < N; ++pair) memset(out->strands + base[(size_t)pair], pair & 1, (size_t)stored[(size_t)pair]);
+    if (records) {  // one record: every hit is in record 0, with its column as it is
+        *records = static_cast<int*>(malloc(sizeof(int) * (size_t)std::max(S, 1LL)));
+        if (!*records) throw std::runtime_error("out of memory for the hit lists");
+        if (p->sep < 0) memset(*records, 0, sizeof(int) * (size_t)S);
+    }
     trace.mark("hits: placed");
     if (S == 0) {
         if (task != EDLIB_TASK_DISTANCE) hit_alignments(task, 0, stored, nullptr, nullptr, nullptr, outAln);
@@ -1139,7 +1150,7 @@ void Pass::hits(long long maxHits, int task, EdlibB200HitAlignments* outAln) {
         hp.at = r.dAt.p;
         hp.room = r.dRoom.p;
         be->launch_hits_place(hp);
-        const HitParams h{nullptr, r.dAt.p, r.dRoom.p, dCols.p, dScores.p};
+        const HitParams h{nullptr, r.dAt.p, r.dRoom.p, dCols.p, dScores.p, sepCodes, p->sep};
         if (ri < seedRuns) {
             be->launch_k1w_hits(window_params(tg, r.jobs, r.numJobs), h, r.nw);
         } else {
@@ -1152,11 +1163,28 @@ void Pass::hits(long long maxHits, int task, EdlibB200HitAlignments* outAln) {
             be->launch_k1_hits(kp, h, r.nw);
         }
     }
-    dCols.download(out->columns, (size_t)S);
     dScores.download(out->scores, (size_t)S);
-    stats.d2hBytes += 8 * S;
     trace.mark("hits: filled");
     if (task != EDLIB_TASK_DISTANCE) hit_alignments(task, S, stored, dBase.p, dCols.p, dScores.p, outAln);
+    if (p->sep >= 0) {  // columns into their records (the starts were mapped slice by slice)
+        DevBuf<int> dRecords(be, (size_t)S);
+        RecordParams rp;
+        memset(&rp, 0, sizeof(rp));
+        rp.stage = REC_HITS;
+        rp.recOff = p->dRecOff.p;
+        rp.numRecords = (int)p->recOff.size() - 1;
+        rp.cols = dCols.p;
+        rp.records = dRecords.p;
+        for (long long lo = 0; lo < S; lo += 1LL << 30) {
+            rp.firstHit = lo;
+            rp.numItems = (int)std::min(S - lo, 1LL << 30);
+            be->launch_record(rp);
+        }
+        dRecords.download(*records, (size_t)S);
+        stats.d2hBytes += 4 * S;
+    }
+    dCols.download(out->columns, (size_t)S);
+    stats.d2hBytes += 8 * S;
 }
 
 // Start locations and edit scripts of the stored hits.  The stored hits are cut into slices of consecutive slots whose
@@ -1225,6 +1253,10 @@ void Pass::hit_alignments(int task, long long S, const std::vector<long long>& s
         hp.starts = dStart.p;
         hp.len = dLen.p;
         hp.err = dErr.p;
+        if (p->sep >= 0) {  // a start lies in its hit's record
+            hp.recOff = p->dRecOff.p;
+            hp.numRecords = (int)p->recOff.size() - 1;
+        }
         std::vector<std::unique_ptr<HitPathClass>> done;
         for (int nw = 1; nw <= 8; ++nw) {
             if (!((classes >> nw) & 1u)) continue;
@@ -1277,6 +1309,18 @@ void Pass::hit_alignments(int task, long long S, const std::vector<long long>& s
             hp.numItems = J;
             be->launch_hit_res(hp);
             done.push_back(std::move(c));
+        }
+        if (p->sep >= 0) {  // starts into their records, while the columns still address the whole target
+            RecordParams rp;
+            memset(&rp, 0, sizeof(rp));
+            rp.stage = REC_STARTS;
+            rp.numItems = span;
+            rp.recOff = p->dRecOff.p;
+            rp.numRecords = (int)p->recOff.size() - 1;
+            rp.firstHit = lo;
+            rp.cols = const_cast<int*>(dCols);
+            rp.starts = dStart.p;
+            be->launch_record(rp);
         }
         be->d2h(out->starts + lo, dStart.p, (size_t)span * sizeof(int));
         stats.d2hBytes += 4LL * span;

@@ -157,6 +157,41 @@ EDLIB_API int edlibB200FindHitAlignments(const char* const* queries, const int* 
 /* Frees the arrays of edlibB200FindHitAlignments and clears the struct. */
 EDLIB_API void edlibB200FreeHitAlignments(EdlibB200HitAlignments* out);
 
+/* The largest multi-record target of edlibB200FindRecordHits, in symbols: the records plus the separators between
+ * them (numRecords - 1 runs of min(config.k, longest query) + 1 symbols).  A larger reference is split by the caller
+ * over several calls. */
+#define EDLIB_B200_MAX_RECORD_TARGET 0x7ffff000
+
+/* Every hit of each query over a reference of several records (chromosomes, plasmids, contigs) in one call.
+ *
+ * The hits of query q on record r are exactly those of edlibB200FindHitAlignments(q, records[r], ..., bothStrands = 0):
+ * column, score, start and script all count from the start of record r, no hit spans two records, and no column outside
+ * a record is reported.  With bothStrands != 0 the hits of rc(q) (the complement table of edlibB200AlignBatchStrands)
+ * follow, with strand 1.  Within a query, hits are ordered by strand (forward first), then by record index, then by
+ * column; counts[i] is exact and the first maxHitsPerQuery hits in that order are stored.  records[h] is the record of
+ * stored hit h; the other arrays are those of EdlibB200HitAlignments, for config.task EDLIB_TASK_DISTANCE, EDLIB_TASK_LOC
+ * or EDLIB_TASK_PATH.
+ *
+ * Accepted: the queries and config that edlibB200FindHits accepts (the task may also be LOC or PATH), numRecords >= 1,
+ * every records[r] non-NULL with recordLengths[r] >= 1, and records plus separators of at most
+ * EDLIB_B200_MAX_RECORD_TARGET symbols (checked before any record byte is read).  The records are laid out in one
+ * target, separated by a code that neither the queries nor the records use: when they use all 256 codes (after
+ * transitive equalities are merged) and there is more than one record, no code is left and the call is refused.
+ * Anything else returns EDLIB_STATUS_ERROR with a message in edlibB200LastError (starting with
+ * "edlibB200FindRecordHits:" for invalid input) and *out left empty; on success the arrays are malloc'd and
+ * edlibB200FreeRecordHits releases them.  edlibB200LastStats reports what edlibB200FindHits reports. */
+typedef struct {
+    EdlibB200HitAlignments aln;  /* as edlibB200FindHitAlignments; columns and starts count from the start of the hit's record */
+    int* records;                /* record index of each stored hit */
+} EdlibB200RecordHits;
+
+EDLIB_API int edlibB200FindRecordHits(const char* const* queries, const int* queryLengths, int numQueries,
+                                      const char* const* records, const int* recordLengths, int numRecords,
+                                      const EdlibAlignConfig config, int bothStrands, long long maxHitsPerQuery,
+                                      EdlibB200RecordHits* out);
+/* Frees the arrays of edlibB200FindRecordHits and clears the struct. */
+EDLIB_API void edlibB200FreeRecordHits(EdlibB200RecordHits* out);
+
 /* A target kept resident on the device.  edlibAlignBatch calls of read sets (HW, short queries, plain equality) whose
  * targets[i] all equal (target, targetLength) of a live handle skip the target's upload, its encoding and the build of
  * its seed index: a caller that aligns many batches to one genome pays them once.  The bytes at `target` must not
