@@ -12,7 +12,7 @@ import re as _re
 from ._ffi import (EDLIB_CIGAR_EXTENDED, EDLIB_CIGAR_STANDARD, EDLIB_STATUS_OK, MODES, TASKS, EdlibLib,
                    product_path)
 
-__all__ = ["align", "align_batch", "align_many", "find_hits", "getNiceAlignment", "library"]
+__all__ = ["align", "align_batch", "align_many", "align_records", "find_hits", "getNiceAlignment", "library"]
 
 _lib = None
 
@@ -111,6 +111,38 @@ def align_batch(queries, targets, mode="NW", task="distance", k=-1, additionalEq
 
 
 align_many = align_batch  # the name SURVEY.md 8f proposes for the batched binding entry
+
+
+def align_records(queries, records, task="distance", k=-1, additionalEqualities=None, strands="forward"):
+    """Each query aligned (HW mode) against a reference of several records (chromosomes, plasmids, contigs) in one
+    call, with the result of its best record: the lowest-index record among those of least edit distance (record 0
+    when none is within k).  Returns one dict per query, that of `align_batch(query, records[r], mode="HW", ...)` for
+    that record r, plus "record": r.  Locations count from the start of the record, and "alphabetLength" covers the
+    query and that record only.
+
+    strands="both": the query and its reverse complement each get their best record; the reverse one is reported only
+    when strictly better, and the dict gains "strand" as for `align_batch`.  The sequence rules are those of
+    `align_batch`."""
+    if strands not in ("forward", "both"):
+        raise ValueError("strands must be 'forward' or 'both'")
+    if task not in TASKS:
+        raise ValueError("task must be 'distance', 'locations' or 'path'")
+    queries, records = list(queries), list(records)
+    if strands == "both" and not all(_is_plain(s) for s in queries + records):
+        raise ValueError("strands='both' needs bytes or ASCII str sequences")
+    mapped, eqs = _map_to_bytes(queries + records, additionalEqualities)
+    both = strands == "both"
+    lib = library()
+    st, res, chosen, strand = lib.align_records(mapped[:len(queries)], mapped[len(queries):], -1 if k is None else k,
+                                                TASKS[task], eqs, both)
+    if st != EDLIB_STATUS_OK:
+        raise Exception("There was an error. (" + lib.lib.edlibB200LastError().decode() + ")")
+    out = [_result(d, True) for d in res]
+    for i, r in enumerate(out):
+        r["record"] = chosen[i]
+        if both:
+            r["strand"] = "-" if strand[i] else "+"
+    return out
 
 
 def find_hits(queries, target, k, strands="forward", max_hits=None, additionalEqualities=None, task="distance"):

@@ -251,6 +251,34 @@ class EdlibLib:
         self.lib.edlibB200FreeRecordHits(C.byref(a))
         return st, out
 
+    def align_records(self, queries, records, k=-1, task=EDLIB_TASK_DISTANCE, equalities=None, both=False,
+                      mode=EDLIB_MODE_HW):
+        """edlibB200AlignRecords: each query against a list of records, the result of its best record.  Returns
+        (status, [dict], [record], [strand] or None) with the dicts of align_batch; status != 0: (status, None, None,
+        None)."""
+        fn = self.lib.edlibB200AlignRecords
+        fn.restype = C.c_int
+        fn.argtypes = [C.POINTER(C.c_char_p), C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int),
+                       C.c_int, AlignConfig, C.c_int, C.POINTER(AlignResult), C.POINTER(C.c_int), C.POINTER(C.c_ubyte)]
+        n, r = len(queries), len(records)
+        cfg, keep = make_config(k, mode, task, equalities)
+        qptr = (C.c_char_p * max(n, 1))(*queries)
+        qlen = (C.c_int * max(n, 1))(*[len(q) for q in queries])
+        rptr = (C.c_char_p * max(r, 1))(*records)
+        rlen = (C.c_int * max(r, 1))(*[len(x) for x in records])
+        res = (AlignResult * max(n, 1))()
+        recs = (C.c_int * max(n, 1))()
+        strands = (C.c_ubyte * max(n, 1))()
+        st = fn(qptr, qlen, n, rptr, rlen, r, cfg, 1 if both else 0, res, recs, strands)
+        del keep
+        if st != EDLIB_STATUS_OK:
+            return st, None, None, None
+        out = []
+        for i in range(n):
+            out.append(result_to_dict(res[i]))
+            self.free(res[i])
+        return st, out, list(recs[:n]), (list(strands[:n]) if both else None)
+
     def _run_batch(self, call, queries, targets, k, mode, task, equalities):
         n = len(queries)
         cfg, keep = make_config(k, mode, task, equalities)

@@ -463,14 +463,33 @@ EDLIB_API void edlibB200FreeCigars(char** cigars, int n) {
     eb::host_parallel_ranges((size_t)n, 16384, free_range);
 }
 
-// What edlibB200FindHits (alignments == false) / edlibB200FindHitAlignments / edlibB200FindRecordHits (records != NULL)
-// refuse (include/edlib_b200.h), or "".  Only lengths are read: a record's bytes are not touched here.
+// The records of edlibB200FindRecordHits / edlibB200AlignRecords.
 struct RecordArgs {
     const char* const* records;
     const int* lengths;
     int n;
-    int gap;  // separator symbols between two records (set here)
+    int gap;  // separator symbols between two records (set by record_input_error)
 };
+
+// What a record call refuses of its records (include/edlib_b200.h), or "", with `at` the message prefix; sets the gap.
+// Only lengths are read: a record's bytes are not touched here.
+static std::string record_input_error(const std::string& at, RecordArgs* records, int k, int longest) {
+    if (records->n < 1) return at + "numRecords must be >= 1";
+    if (!records->records || !records->lengths) return at + "no records";
+    // an alignment that crosses a separator of gap symbols costs more than k (if k >= 0) and more than any query's length
+    records->gap = (k < 0 ? longest : std::min(k, longest)) + 1;
+    long long total = (long long)(records->n - 1) * records->gap;
+    for (int r = 0; r < records->n; ++r) {
+        if (!records->records[r] || records->lengths[r] < 1) return at + "every record must be non-NULL with at least one symbol";
+        total += records->lengths[r];
+    }
+    if (total > EDLIB_B200_MAX_RECORD_TARGET)
+        return at + "the records and their separators exceed EDLIB_B200_MAX_RECORD_TARGET symbols";
+    return std::string();
+}
+
+// What edlibB200FindHits (alignments == false) / edlibB200FindHitAlignments / edlibB200FindRecordHits (records != NULL)
+// refuse (include/edlib_b200.h), or "".
 static std::string hits_input_error(const char* entry, bool alignments, const char* const* queries, const int* queryLengths,
                                     int numQueries, const char* target, int targetLength, RecordArgs* records,
                                     const EdlibAlignConfig& config, int bothStrands, long long maxHits) {
@@ -492,18 +511,7 @@ static std::string hits_input_error(const char* entry, bool alignments, const ch
         longest = std::max(longest, queryLengths[i]);
     }
     if (!records) return std::string();
-    if (records->n < 1) return at + "numRecords must be >= 1";
-    if (!records->records || !records->lengths) return at + "no records";
-    // an alignment that crosses a separator of gap symbols costs more than k and more than any query's length
-    records->gap = std::min(config.k, longest) + 1;
-    long long total = (long long)(records->n - 1) * records->gap;
-    for (int r = 0; r < records->n; ++r) {
-        if (!records->records[r] || records->lengths[r] < 1) return at + "every record must be non-NULL with at least one symbol";
-        total += records->lengths[r];
-    }
-    if (total > EDLIB_B200_MAX_RECORD_TARGET)
-        return at + "the records and their separators exceed EDLIB_B200_MAX_RECORD_TARGET symbols";
-    return std::string();
+    return record_input_error(at, records, config.k, longest);
 }
 
 // The hit entries: `out` (never NULL here) is cleared, then filled on success; on failure nothing stays allocated.
@@ -595,6 +603,64 @@ EDLIB_API void edlibB200FreeRecordHits(EdlibB200RecordHits* out) {
     eb::free_hit_alignments(&out->aln);
     free(out->records);
     out->records = nullptr;
+}
+
+// What edlibB200AlignRecords refuses (include/edlib_b200.h), or "".
+static std::string align_records_error(const char* const* queries, const int* queryLengths, int numQueries,
+                                       RecordArgs* records, const EdlibAlignConfig& config, int bothStrands,
+                                       const EdlibAlignResult* results, const int* recordsOut, const unsigned char* strandsOut) {
+    const std::string at = "edlibB200AlignRecords: ";
+    if (numQueries < 0) return at + "numQueries < 0";
+    if (numQueries > 0 && (!queries || !queryLengths)) return at + "no queries";
+    if (numQueries > 0 && !results) return at + "results is NULL";
+    if (numQueries > 0 && !recordsOut) return at + "recordsOut is NULL";
+    if (bothStrands && numQueries > 0 && !strandsOut) return at + "strandsOut is NULL";
+    if (bothStrands && numQueries > 0x3fffffff) return at + "too many queries for both strands";
+    if (config.mode != EDLIB_MODE_HW) return at + "mode must be EDLIB_MODE_HW";
+    if (config.task != EDLIB_TASK_DISTANCE && config.task != EDLIB_TASK_LOC && config.task != EDLIB_TASK_PATH)
+        return at + "task must be EDLIB_TASK_DISTANCE, EDLIB_TASK_LOC or EDLIB_TASK_PATH";
+    if (config.additionalEqualitiesLength > 0 && !config.additionalEqualities) return at + "no equality pairs";
+    int longest = 0;
+    for (int i = 0; i < numQueries; ++i) {
+        if (queryLengths[i] < 0 || (queryLengths[i] > 0 && !queries[i])) return at + "every query must be non-NULL with a length >= 0";
+        longest = std::max(longest, queryLengths[i]);
+    }
+    return record_input_error(at, records, config.k, longest);
+}
+
+EDLIB_API int edlibB200AlignRecords(const char* const* queries, const int* queryLengths, int numQueries,
+                                    const char* const* records, const int* recordLengths, int numRecords,
+                                    const EdlibAlignConfig config, int bothStrands, EdlibAlignResult* results,
+                                    int* recordsOut, unsigned char* strandsOut) {
+    std::lock_guard<std::mutex> lock(g_mu);
+    eb::Engine* e = engine_locked();
+    if (!e) {  // no usable device: there is no CPU path
+        if (results && numQueries > 0) eb::fail_results(results, numQueries);
+        return EDLIB_STATUS_ERROR;
+    }
+    t_lastEngine = e;
+    RecordArgs ra{records, recordLengths, numRecords, 0};
+    const std::string bad = align_records_error(queries, queryLengths, numQueries, &ra, config, bothStrands, results,
+                                                recordsOut, strandsOut);
+    if (!bad.empty()) {
+        e->lastError = bad;
+        if (results && numQueries > 0) eb::fail_results(results, numQueries);
+        return EDLIB_STATUS_ERROR;
+    }
+    if (numQueries == 0) return EDLIB_STATUS_OK;
+    // one target laid out from the records: its length, no host pointer
+    int targetLength = (ra.n - 1) * ra.gap;
+    for (int r = 0; r < ra.n; ++r) targetLength += ra.lengths[r];
+    const std::vector<const char*> targets((size_t)numQueries, nullptr);
+    const std::vector<int> targetLengths((size_t)numQueries, targetLength);
+    eb::BatchInput in{queries, queryLengths, targets.data(), targetLengths.data(), numQueries, config};
+    in.strands = bothStrands != 0;
+    in.records = ra.records;
+    in.recordLengths = ra.lengths;
+    in.numRecords = ra.n;
+    in.recordGap = ra.gap;
+    in.bestRecord = true;
+    return e->align_batch(in, results, in.strands ? strandsOut : nullptr, recordsOut);
 }
 
 EDLIB_API void edlibB200LastStats(EdlibB200Stats* s) {

@@ -170,6 +170,9 @@ Prepared* Engine::take_prepared(const BatchInput& in) {
     p->dRecOff.reset();
     p->recGap = 0;
     p->sep = -1;
+    p->bestRecord = in.bestRecord;
+    p->record.clear();
+    p->dMasks.reset();
     p->computed = false;
     p->classified = false;
     p->groups.clear();
@@ -415,26 +418,28 @@ Prepared* Engine::prepare(const BatchInput& in) {
         for (int i = 0; i < N; i += qstep)
             if (p->qlen[i] > 65536) longQueries.push_back(i);
 
-        // byte-presence sets: one per query, one per distinct target, one union for the batch.  Queries are
-        // implicit work items of the kernel; explicit ones (at most 65536 bytes each) are only needed for
-        // the targets and for the pieces of longer queries.
+        // byte-presence sets: one per query, one per distinct target (a record target: one per record), one union for
+        // the batch.  Queries are implicit work items of the kernel; explicit ones (at most 65536 bytes each) are only
+        // needed for the targets and for the pieces of longer queries.
         std::vector<MaskItem> items;
         auto add_items = [&](uint64_t off, int len, int dst) {
             for (int s0 = 0; s0 < len; s0 += 65536) items.push_back(MaskItem{off + (uint64_t)s0, std::min(65536, len - s0), dst});
         };
         for (int i : longQueries) add_items(p->qoff[i], p->qlen[i], i);
         if (numRec > 0) {  // the records only: no separator byte enters a presence set
-            for (int r = 0; r < numRec; ++r) add_items(p->tg[0].off + (uint64_t)p->recOff[(size_t)r], in.recordLengths[r], N);
+            for (int r = 0; r < numRec; ++r) add_items(p->tg[0].off + (uint64_t)p->recOff[(size_t)r], in.recordLengths[r], N + r);
         } else {
             for (int t = 0; t < T; ++t) add_items(p->tg[t].off, p->tg[t].len, N + t);
         }
+        // (a record target of the hit search: set N, record 0's; its alphabet lengths are not reported)
         HostBuf<int> tset(be, (size_t)N);
         parallel_ranges((size_t)N, 65536, [&](size_t lo, size_t hi) {
             for (size_t i = lo; i < hi; ++i) tset[i] = N + p->tidx[i];
         });
-        const int unionSet = N + T;
-        DevBuf<uint32_t> dMasks(be, (size_t)(N + T + 1) * 8);
-        be->zero(dMasks.p, (size_t)(N + T + 1) * 8 * sizeof(uint32_t));
+        const int numSets = std::max(T, numRec);
+        const int unionSet = N + numSets;
+        DevBuf<uint32_t> dMasks(be, (size_t)(N + numSets + 1) * 8);
+        be->zero(dMasks.p, (size_t)(N + numSets + 1) * 8 * sizeof(uint32_t));
         DevBuf<MaskItem> dItems(be, items.size());
         if (!items.empty()) dItems.upload(items.data(), items.size());
         {
@@ -455,16 +460,22 @@ Prepared* Engine::prepare(const BatchInput& in) {
             if (mp.numItems + mp.numQueries > 0) be->launch_mask(mp);
         }
         DevBuf<int> dTset(be, N), dAlpha(be, N);
-        dTset.upload(tset.p, N);
         trace.mark("prepare: mask items");
-        be->launch_alpha_len(dMasks.p, nullptr, dTset.p, N, dAlpha.p);
+        if (!in.bestRecord) {  // a best-record batch: once the record of each pair is known (Pass::pick_records)
+            dTset.upload(tset.p, N);
+            be->launch_alpha_len(dMasks.p, nullptr, dTset.p, N, dAlpha.p);
+        }
         classify(p);  // host work while the upload and the alphabet kernels run
         trace.mark("prepare: classification");
-        p->alphaLen.resize(N);
-        dAlpha.download(p->alphaLen.data(), N);
+        if (!in.bestRecord) {
+            p->alphaLen.resize(N);
+            dAlpha.download(p->alphaLen.data(), N);
+            stats.d2hBytes += (long long)N * 4;
+        }
         uint32_t uni[8];
         be->d2h(uni, dMasks.p + (size_t)unionSet * 8, sizeof(uni));
-        stats.d2hBytes += (long long)N * 4 + 32;
+        stats.d2hBytes += 32;
+        if (in.bestRecord) p->dMasks.swap(dMasks);
         trace.mark("prepare: alphabet lengths back");
 
         // dense codes in ascending byte order; absent bytes (padding) map to code 0
@@ -531,8 +542,9 @@ Prepared* Engine::prepare(const BatchInput& in) {
         // wildcard (its row and column of the equality table stay 0)
         if (numRec > 1) {
             if (p->ncodes >= 256)
-                throw std::runtime_error("edlibB200FindRecordHits: the queries and records use all 256 codes: none is left for "
-                                         "the separator between records");
+                throw std::runtime_error(std::string(in.bestRecord ? "edlibB200AlignRecords" : "edlibB200FindRecordHits") +
+                                         ": the queries and records use all 256 codes: none is left for the separator "
+                                         "between records");
             p->sep = p->ncodes++;
             if (anyEq) {
                 const int s0 = p->sep, s1 = p->ncodes;
@@ -758,6 +770,7 @@ void Engine::compute(Prepared* p) {
     } else {
         ps.collect_ends(nullptr);
     }
+    if (p->bestRecord) ps.pick_records();
     if (p->strands) ps.pick_strands();
     trace.mark("compute: end locations");
     ps.start_locations();
@@ -878,6 +891,7 @@ void Engine::release(Prepared* p) {
     p->dQlen.reset();
     p->dEqtab.reset();
     p->dRecOff.reset();
+    p->dMasks.reset();
     p->computed = false;
     if (spare_) {
         delete p;
@@ -942,7 +956,14 @@ void Engine::strands_of(const Prepared* p, unsigned char* strands) const {
     memcpy(strands, p->strand.data(), p->strand.size());
 }
 
-int Engine::align_batch(const BatchInput& in, EdlibAlignResult* results, unsigned char* strands) {
+void Engine::records_of(const Prepared* p, int* records) const {
+    if (!p->bestRecord) throw std::runtime_error("records requested from a batch not prepared as a best-record batch");
+    if (!p->computed) throw std::runtime_error("records requested from a batch that was not (successfully) computed");
+    const int n = p->strands ? p->N / 2 : p->N;
+    for (int i = 0; i < n; ++i) records[i] = p->record[(size_t)(p->strands ? 2 * i + p->strand[(size_t)i] : i)];
+}
+
+int Engine::align_batch(const BatchInput& in, EdlibAlignResult* results, unsigned char* strands, int* records) {
     Prepared* p = nullptr;
     stats = EngineStats();
     statsPending_ = false;
@@ -952,6 +973,7 @@ int Engine::align_batch(const BatchInput& in, EdlibAlignResult* results, unsigne
         compute(p);
         materialize(p, results);  // releases what it built when it fails
         if (strands) strands_of(p, strands);
+        if (records) records_of(p, records);
         release(p);
         return EDLIB_STATUS_OK;
     } catch (const std::exception& e) {
@@ -1052,7 +1074,8 @@ struct StreamJob {
 bool Engine::align_streamed(const BatchInput& in, EdlibAlignResult* results) {
     Backend* be = be_;
     const int N = in.numPairs;
-    if (in.config.mode != EDLIB_MODE_HW || N < tun.streamMinPairs || !tun.deviceStage || in.strands) return false;
+    if (in.config.mode != EDLIB_MODE_HW || N < tun.streamMinPairs || !tun.deviceStage || in.strands || in.numRecords > 0)
+        return false;
     if (in.config.additionalEqualities && in.config.additionalEqualitiesLength > 0) return false;
     if (tun.filterSeedK <= 0 || tun.filterSeedLevels <= 0) return false;
     const char* tptr = in.targets[0];

@@ -116,12 +116,16 @@ struct BatchInput {
     int numPairs;
     EdlibAlignConfig config;
     bool strands = false;  // align every query and its reverse complement, report the better strand (Prepared::strands)
-    // A record target (edlibB200FindRecordHits; targets[i] == nullptr, targetLengths[i] == the laid-out length): the
-    // records in order, each but the last followed by recordGap separator columns.  numRecords == 0: plain targets.
+    // A record target (edlibB200FindRecordHits, edlibB200AlignRecords; targets[i] == nullptr, targetLengths[i] == the
+    // laid-out length): the records in order, each but the last followed by recordGap separator columns.  numRecords
+    // == 0: plain targets.
     const char* const* records = nullptr;
     const int* recordLengths = nullptr;
     int numRecords = 0;
     int recordGap = 0;
+    // edlibB200AlignRecords: each pair's result is that of its best record (Pass::pick_records), whose index
+    // Engine::records_of reports
+    bool bestRecord = false;
 };
 
 struct EngineTunables {
@@ -192,10 +196,11 @@ class Engine {
 public:
     explicit Engine(Backend* be);
     ~Engine();
-    // One-shot: prepare + compute + materialise (and, for a strand batch, the chosen strand per read into `strands`).
-    // Returns EDLIB_STATUS_OK / EDLIB_STATUS_ERROR.
-    int align_batch(const BatchInput& in, EdlibAlignResult* results, unsigned char* strands = nullptr);
+    // One-shot: prepare + compute + materialise (and, for a strand batch, the chosen strand per read into `strands`; for
+    // a best-record batch, the record of each result into `records`).  Returns EDLIB_STATUS_OK / EDLIB_STATUS_ERROR.
+    int align_batch(const BatchInput& in, EdlibAlignResult* results, unsigned char* strands = nullptr, int* records = nullptr);
     void strands_of(const Prepared* p, unsigned char* strands) const;  // a computed strand batch: 1 where the reverse strand won
+    void records_of(const Prepared* p, int* records) const;  // a computed best-record batch: the record of each result
 
     // Staged form (bench "inputs resident in HBM" measurement, multi-GPU shards):
     Prepared* prepare(const BatchInput& in);                 // upload, alphabet, encode

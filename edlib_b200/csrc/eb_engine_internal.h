@@ -257,6 +257,11 @@ struct DevBuf {
     }
     void upload(const T* src, size_t count) { be->h2d(p, src, count * sizeof(T)); }
     void download(T* dst, size_t count) { be->d2h(dst, p, count * sizeof(T)); }
+    void swap(DevBuf& o) {
+        std::swap(be, o.be);
+        std::swap(p, o.p);
+        std::swap(n, o.n);
+    }
 };
 
 // Growable array in staging memory of the backend (pinned on CUDA): result arrays the device writes with
@@ -379,6 +384,11 @@ public:
     DevBuf<int> dRecOff;
     int recGap = 0;
     int sep = -1;
+    // A best-record batch (BatchInput::bestRecord): the presence sets of prepare (pair i: set i, record r: set N + r),
+    // kept until Pass::pick_records has chosen the record of each pair, `record`, and alphaLen follows from them.
+    bool bestRecord = false;
+    std::vector<int> record;
+    DevBuf<uint32_t> dMasks;
 
     // classification (Engine::classify): pairs per (target, word class) for the lane kernels, the rest
     struct Part {
@@ -681,6 +691,10 @@ struct Pass {
     // After the end locations: per read of a strand batch, the winning strand (Prepared::strand); the loser's result
     // becomes "no alignment", so that start locations and paths are only computed for winners.
     void pick_strands();
+    // After the end locations of a best-record batch, before pick_strands: per pair, the first record that holds one of
+    // its end columns (Prepared::record), its end columns kept and counted from that record's start; then every pair
+    // is rebased onto its record (one Target per record, tidx / tlen) and its alphabet length taken over that record.
+    void pick_records();
 
     // Outcome of the reads `cand` (indices into `list`) of a window stage, with thresholds thr[i] (< 0: the stage left
     // the read out, it goes on), their plans on the device and the records of their swept windows: the reduction

@@ -358,6 +358,68 @@ void Pass::pick_strands() {
     });
 }
 
+// The distance over the record target is the least distance over the records, and its end columns within a record are
+// exactly that record's (DESIGN.md section 3).  A separator column may tie the best score; the last column of the
+// record before it then does too, so a pair with a distance always keeps a record column.  The first one names the
+// lowest record of least distance; its columns follow in ascending order, the other records' columns after them.
+void Pass::pick_records() {
+    const int R = (int)p->recOff.size() - 1;
+    const int* recOff = p->recOff.data();
+    const int gap = p->recGap;
+    p->record.assign((size_t)N, 0);
+    std::atomic<int> lost(0);
+    parallel_ranges((size_t)N, 65536, [&](size_t lo, size_t hi) {
+        for (size_t i = lo; i < hi; ++i) {
+            if (p->ed[i] < 0) continue;  // no alignment within k (or an empty query): every record ties, record 0
+            int* e = p->endPool.data() + p->endStart[i];
+            const int c = p->endCount[i];
+            int kept = 0, r = -1, x = 0;
+            if (c > 0 && e[0] < 0) kept = x = 1;  // the leading -1 of the reference's rule stays
+            for (; x < c; ++x) {
+                const int col = e[x];
+                if (r < 0) {
+                    const int s = (int)(std::upper_bound(recOff, recOff + R, col) - recOff) - 1;  // last recOff[s] <= col
+                    if (col >= recOff[s + 1] - gap) continue;  // a separator column
+                    r = s;
+                } else if (col >= recOff[r + 1] - gap) {
+                    break;  // past the record: the rest are separator columns and later records
+                }
+                e[kept++] = col - recOff[r];
+            }
+            if (r < 0) {
+                lost.store(1, std::memory_order_relaxed);
+                continue;
+            }
+            p->record[i] = r;
+            p->endCount[i] = kept;
+        }
+    });
+    if (lost.load()) throw std::runtime_error("internal: a best-record pair has no end column in a record");
+    // every pair onto its record: start locations and paths see a batch whose pair i has target tg[record[i]]
+    std::vector<Target> recs((size_t)R);
+    for (int r = 0; r < R; ++r) recs[(size_t)r] = Target{nullptr, recOff[r + 1] - recOff[r] - gap, p->tg[0].off + (uint64_t)recOff[r]};
+    p->tg.swap(recs);
+    HostBuf<int> tset(be, (size_t)N);
+    parallel_ranges((size_t)N, 65536, [&](size_t lo, size_t hi) {
+        for (size_t i = lo; i < hi; ++i) {
+            const int r = p->record[i];
+            p->tidx[i] = r;
+            p->tlen[i] = p->tg[(size_t)r].len;
+            tset[i] = N + r;
+        }
+    });
+    // alphabet lengths over the query and its record (prepare's presence sets: pair i in set i, record r in N + r)
+    DevBuf<int> dTset(be, (size_t)N), dAlpha(be, (size_t)N);
+    dTset.upload(tset.p, (size_t)N);
+    be->launch_alpha_len(p->dMasks.p, nullptr, dTset.p, N, dAlpha.p);
+    p->alphaLen.resize((size_t)N);
+    dAlpha.download(p->alphaLen.data(), (size_t)N);
+    p->dMasks.reset();
+    stats.h2dBytes += 4LL * N;
+    stats.d2hBytes += 4LL * N;
+    trace.mark("records: best record per pair");
+}
+
 // =============================================================================================
 // Start locations and paths of short queries (<= 256 rows) driven from the device.  A read set needs one reversed
 // sweep per end location and one matrix-storing sweep + traceback per read: millions of tiny jobs.  Their

@@ -192,6 +192,33 @@ EDLIB_API int edlibB200FindRecordHits(const char* const* queries, const int* que
 /* Frees the arrays of edlibB200FindRecordHits and clears the struct. */
 EDLIB_API void edlibB200FreeRecordHits(EdlibB200RecordHits* out);
 
+/* Each query aligned (HW mode) against a reference of several records in one call, with the result of its best record.
+ *
+ * For query q let A(r) = edlibAlign(q, records[r], config).  The best record r* is the lowest index among the records
+ * of least distance, where "none within k" (-1) counts as larger than any distance; so when no record has an alignment
+ * within k, and for an empty query, r* = 0.  results[i] is A(r*) in every field: alphabetLength counts the distinct
+ * bytes of q and records[r*] only, and endLocations (with the reference's leading -1 where it gives one),
+ * startLocations and alignment count from the start of records[r*].  recordsOut[i] = r*.
+ *
+ * bothStrands != 0: q and rc(q) (the complement table of edlibB200AlignBatchStrands) each get their best record, and
+ * the strand is chosen by the rule of edlibB200AlignBatchStrands (the reverse strand only when strictly better);
+ * strandsOut[i] receives it, and a reverse result is edlibAlign(rc(q), records[r*], config).
+ *
+ * Accepted: config.mode EDLIB_MODE_HW with any task, k (-1 included) and additional equalities; queries of any length
+ * (0 included); numRecords >= 1, every records[r] non-NULL with recordLengths[r] >= 1; results and recordsOut (and
+ * strandsOut with bothStrands) of numQueries entries.  The records are laid out in one target, each but the last
+ * followed by g separator symbols, g = min(k, longest query) + 1 (longest query + 1 for k < 0); records plus
+ * separators must not exceed EDLIB_B200_MAX_RECORD_TARGET symbols, which is checked before any record byte is read.
+ * As for edlibB200FindRecordHits, a call of several records whose queries and records use all 256 codes is refused.
+ * One record needs no separator: the results are those of edlibAlignBatch against it.  Errors return
+ * EDLIB_STATUS_ERROR with a message in edlibB200LastError (starting with "edlibB200AlignRecords:" for invalid input)
+ * and no arrays allocated; results are freed as those of edlibAlignBatch.  edlibB200LastStats reports the distance
+ * pass, as for edlibAlignBatch. */
+EDLIB_API int edlibB200AlignRecords(const char* const* queries, const int* queryLengths, int numQueries,
+                                    const char* const* records, const int* recordLengths, int numRecords,
+                                    const EdlibAlignConfig config, int bothStrands,
+                                    EdlibAlignResult* results, int* recordsOut, unsigned char* strandsOut);
+
 /* A target kept resident on the device.  edlibAlignBatch calls of read sets (HW, short queries, plain equality) whose
  * targets[i] all equal (target, targetLength) of a live handle skip the target's upload, its encoding and the build of
  * its seed index: a caller that aligns many batches to one genome pays them once.  The bytes at `target` must not
