@@ -12,7 +12,8 @@ import re as _re
 from ._ffi import (EDLIB_CIGAR_EXTENDED, EDLIB_CIGAR_STANDARD, EDLIB_STATUS_OK, MODES, TASKS, EdlibLib,
                    product_path)
 
-__all__ = ["align", "align_batch", "align_many", "align_records", "find_hits", "getNiceAlignment", "library"]
+__all__ = ["align", "align_batch", "align_many", "align_records", "find_hits", "find_pair_hits", "getNiceAlignment",
+           "library"]
 
 _lib = None
 
@@ -186,6 +187,44 @@ def find_hits(queries, target, k, strands="forward", max_hits=None, additionalEq
         st, res = lib.find_hits(queries, targets[0], k, both, cap, eqs)
     else:
         st, res = lib.find_hit_alignments(queries, targets[0], k, both, cap, eqs, TASKS[task])
+    if st != EDLIB_STATUS_OK:
+        raise Exception("There was an error. (" + lib.lib.edlibB200LastError().decode() + ")")
+    for r in res:
+        if both:
+            r["hits"] = [h[:-1] + ("-" if h[-1] else "+",) for h in r["hits"]]
+        if "alignments" in r:
+            r["cigars"] = [lib.cigar(a, EDLIB_CIGAR_EXTENDED) for a in r.pop("alignments")]
+    return res
+
+
+def find_pair_hits(queries, targets, k, strands="forward", max_hits=None, additionalEqualities=None, task="distance"):
+    """Every place where queries[i] occurs in its own targets[i] with at most k edits, for every pair i in one call
+    (HW mode; queries of 1..256 symbols): a read's candidate region, its amplicon, the locus a guide is assigned to.
+
+    Returns one dict per pair, that of `find_hits([queries[i]], targets[i], ...)` for its one query: {"count", "hits":
+    [(column, score[, "+"/"-"]), ...]} and, for task "locations" / "path", "starts" / "cigars"; columns and starts count
+    from the start of targets[i].  An empty target has no hits.  The sequence rules and target sharing are those of
+    `align_batch`: repeating the same object shares its upload, and many pairs over one target are searched together."""
+    if strands not in ("forward", "both"):
+        raise ValueError("strands must be 'forward' or 'both'")
+    if task not in ("distance", "locations", "path"):
+        raise ValueError("task must be 'distance', 'locations' or 'path'")
+    queries, tlist = list(queries), list(targets)
+    if len(queries) != len(tlist):
+        raise ValueError("queries and targets must have the same length")
+    distinct, index = [], {}
+    for t in tlist:
+        if id(t) not in index:
+            index[id(t)] = len(distinct)
+            distinct.append(t)
+    if strands == "both" and not all(_is_plain(s) for s in queries + distinct):
+        raise ValueError("strands='both' needs bytes or ASCII str sequences")
+    mapped, eqs = _map_to_bytes(queries + distinct, additionalEqualities)
+    qs, ts = mapped[:len(queries)], mapped[len(queries):]
+    both = strands == "both"
+    cap = (1 << 62) if max_hits is None else max_hits
+    lib = library()
+    st, res = lib.find_pair_hits(qs, [ts[index[id(t)]] for t in tlist], k, both, cap, eqs, TASKS[task])
     if st != EDLIB_STATUS_OK:
         raise Exception("There was an error. (" + lib.lib.edlibB200LastError().decode() + ")")
     for r in res:

@@ -226,6 +226,35 @@ class EdlibLib:
         self.lib.edlibB200FreeHitAlignments(C.byref(a))
         return st, out
 
+    def find_pair_hits(self, queries, targets, k, both=False, max_hits=(1 << 62), equalities=None,
+                       task=EDLIB_TASK_DISTANCE, mode=EDLIB_MODE_HW):
+        """edlibB200FindPairHits: query i searched in targets[i] only (repeat the SAME bytes object to share a target).
+        Returns (status, [dict]) as find_hit_alignments, one dict per pair; status != 0: (status, None)."""
+        fn = self.lib.edlibB200FindPairHits
+        fn.restype = C.c_int
+        fn.argtypes = [C.POINTER(C.c_char_p), C.POINTER(C.c_int), C.POINTER(C.c_char_p), C.POINTER(C.c_int), C.c_int,
+                       AlignConfig, C.c_int, C.c_longlong, C.POINTER(HitAlignments)]
+        self.lib.edlibB200FreeHitAlignments.restype = None
+        self.lib.edlibB200FreeHitAlignments.argtypes = [C.POINTER(HitAlignments)]
+        n = len(queries)
+        cfg, keep = make_config(k, mode, task, equalities)
+        qptr = (C.c_char_p * max(n, 1))(*queries)
+        qlen = (C.c_int * max(n, 1))(*[len(q) for q in queries])
+        bufs = {}  # one buffer per distinct object: identical objects share a pointer, hence a target
+        for t in targets:
+            if id(t) not in bufs:
+                bufs[id(t)] = C.create_string_buffer(bytes(t), max(len(t), 1))
+        tptr = (C.c_char_p * max(n, 1))(*[C.cast(bufs[id(t)], C.c_char_p) for t in targets])
+        tlen = (C.c_int * max(n, 1))(*[len(t) for t in targets])
+        a = HitAlignments()
+        st = fn(qptr, qlen, tptr, tlen, n, cfg, 1 if both else 0, max_hits, C.byref(a))
+        del keep, bufs
+        if st != EDLIB_STATUS_OK:
+            return st, None
+        out = _hit_dicts(a, n, both, None)
+        self.lib.edlibB200FreeHitAlignments(C.byref(a))
+        return st, out
+
     def find_record_hits(self, queries, records, k, both=False, max_hits=(1 << 62), equalities=None,
                          task=EDLIB_TASK_DISTANCE, mode=EDLIB_MODE_HW):
         """edlibB200FindRecordHits over a list of records.  Returns (status, [dict]) as find_hit_alignments, with

@@ -488,38 +488,48 @@ static std::string record_input_error(const std::string& at, RecordArgs* records
     return std::string();
 }
 
+// The per-pair targets of edlibB200FindPairHits.
+struct PairArgs {
+    const char* const* targets;
+    const int* lengths;
+};
+
 // What edlibB200FindHits (alignments == false) / edlibB200FindHitAlignments / edlibB200FindRecordHits (records != NULL)
-// refuse (include/edlib_b200.h), or "".
+// / edlibB200FindPairHits (pairs != NULL, one query per pair) refuse (include/edlib_b200.h), or "".
 static std::string hits_input_error(const char* entry, bool alignments, const char* const* queries, const int* queryLengths,
                                     int numQueries, const char* target, int targetLength, RecordArgs* records,
-                                    const EdlibAlignConfig& config, int bothStrands, long long maxHits) {
+                                    const PairArgs* pairs, const EdlibAlignConfig& config, int bothStrands, long long maxHits) {
     const std::string at = std::string(entry) + ": ";
-    if (numQueries < 0) return at + "numQueries < 0";
+    if (numQueries < 0) return at + (pairs ? "numPairs < 0" : "numQueries < 0");
     if (numQueries > 0 && (!queries || !queryLengths)) return at + "no queries";
-    if (bothStrands && numQueries > 0x3fffffff) return at + "too many queries for both strands";
-    if (!records && (!target || targetLength < 1)) return at + "the target must have at least one symbol";
+    if (bothStrands && numQueries > 0x3fffffff) return at + (pairs ? "too many pairs for both strands" : "too many queries for both strands");
+    if (pairs && numQueries > 0 && (!pairs->targets || !pairs->lengths)) return at + "no targets";
+    if (!records && !pairs && (!target || targetLength < 1)) return at + "the target must have at least one symbol";
     if (config.mode != EDLIB_MODE_HW) return at + "mode must be EDLIB_MODE_HW";
     if (!alignments && config.task != EDLIB_TASK_DISTANCE) return at + "task must be EDLIB_TASK_DISTANCE";
     if (alignments && config.task != EDLIB_TASK_DISTANCE && config.task != EDLIB_TASK_LOC && config.task != EDLIB_TASK_PATH)
         return at + "task must be EDLIB_TASK_DISTANCE, EDLIB_TASK_LOC or EDLIB_TASK_PATH";
     if (config.k < 0) return at + "k must be >= 0";
-    if (maxHits < 0) return at + "maxHitsPerQuery must be >= 0";
+    if (maxHits < 0) return at + (pairs ? "maxHitsPerPair must be >= 0" : "maxHitsPerQuery must be >= 0");
     if (config.additionalEqualitiesLength > 0 && !config.additionalEqualities) return at + "no equality pairs";
     int longest = 0;
     for (int i = 0; i < numQueries; ++i) {
         if (!queries[i] || queryLengths[i] < 1 || queryLengths[i] > 256) return at + "query lengths must be 1 .. 256";
         longest = std::max(longest, queryLengths[i]);
+        if (pairs && (pairs->lengths[i] < 0 || (pairs->lengths[i] > 0 && !pairs->targets[i])))
+            return at + "every target length must be >= 0, with a non-NULL target when it is > 0";
     }
     if (!records) return std::string();
     return record_input_error(at, records, config.k, longest);
 }
 
 // The hit entries: `out` (never NULL here) is cleared, then filled on success; on failure nothing stays allocated.
-// records: a record call (edlibB200FindRecordHits), whose record of each stored hit goes to *recordsOut.
+// records: a record call (edlibB200FindRecordHits), whose record of each stored hit goes to *recordsOut.  pairs: a pair
+// call (edlibB200FindPairHits), query i searched in pairs->targets[i] only.
 static int find_hits_entry(const char* entry, bool alignments, bool outNull, const char* const* queries,
                            const int* queryLengths, int numQueries, const char* target, int targetLength,
-                           RecordArgs* records, const EdlibAlignConfig& config, int bothStrands, long long maxHitsPerQuery,
-                           EdlibB200HitAlignments* out, int** recordsOut) {
+                           RecordArgs* records, const PairArgs* pairs, const EdlibAlignConfig& config, int bothStrands,
+                           long long maxHitsPerQuery, EdlibB200HitAlignments* out, int** recordsOut) {
     std::lock_guard<std::mutex> lock(g_mu);
     eb::Engine* e = engine_locked();
     memset(out, 0, sizeof(*out));
@@ -528,7 +538,7 @@ static int find_hits_entry(const char* entry, bool alignments, bool outNull, con
     t_lastEngine = e;
     const std::string bad = outNull ? std::string(entry) + (alignments ? ": out is NULL" : ": hits is NULL")
                                     : hits_input_error(entry, alignments, queries, queryLengths, numQueries, target,
-                                                       targetLength, records, config, bothStrands, maxHitsPerQuery);
+                                                       targetLength, records, pairs, config, bothStrands, maxHitsPerQuery);
     if (!bad.empty()) {
         e->lastError = bad;
         return EDLIB_STATUS_ERROR;
@@ -548,9 +558,10 @@ static int find_hits_entry(const char* entry, bool alignments, bool outNull, con
         for (int r = 0; r < records->n; ++r) targetLength += records->lengths[r];
         target = nullptr;
     }
-    const std::vector<const char*> targets((size_t)numQueries, target);
-    const std::vector<int> targetLengths((size_t)numQueries, targetLength);
-    eb::BatchInput in{queries, queryLengths, targets.data(), targetLengths.data(), numQueries, config};
+    const std::vector<const char*> targets(pairs ? 0 : (size_t)numQueries, target);
+    const std::vector<int> targetLengths(pairs ? 0 : (size_t)numQueries, targetLength);
+    eb::BatchInput in{queries, queryLengths, pairs ? pairs->targets : targets.data(),
+                      pairs ? pairs->lengths : targetLengths.data(), numQueries, config};
     in.strands = bothStrands != 0;
     if (records) {
         in.records = records->records;
@@ -566,7 +577,7 @@ EDLIB_API int edlibB200FindHits(const char* const* queries, const int* queryLeng
                                 EdlibB200Hits* hits) {
     EdlibB200HitAlignments out;
     const int st = find_hits_entry("edlibB200FindHits", false, !hits, queries, queryLengths, numQueries, target,
-                                   targetLength, nullptr, config, bothStrands, maxHitsPerQuery, &out, nullptr);
+                                   targetLength, nullptr, nullptr, config, bothStrands, maxHitsPerQuery, &out, nullptr);
     if (hits) *hits = out.hits;  // task DISTANCE: nothing else was allocated
     return st;
 }
@@ -580,7 +591,7 @@ EDLIB_API int edlibB200FindHitAlignments(const char* const* queries, const int* 
                                          int bothStrands, long long maxHitsPerQuery, EdlibB200HitAlignments* out) {
     EdlibB200HitAlignments scratch;
     return find_hits_entry("edlibB200FindHitAlignments", true, !out, queries, queryLengths, numQueries, target,
-                           targetLength, nullptr, config, bothStrands, maxHitsPerQuery, out ? out : &scratch, nullptr);
+                           targetLength, nullptr, nullptr, config, bothStrands, maxHitsPerQuery, out ? out : &scratch, nullptr);
 }
 
 EDLIB_API void edlibB200FreeHitAlignments(EdlibB200HitAlignments* out) {
@@ -595,7 +606,16 @@ EDLIB_API int edlibB200FindRecordHits(const char* const* queries, const int* que
     EdlibB200RecordHits* o = out ? out : &scratch;
     RecordArgs ra{records, recordLengths, numRecords, 0};
     return find_hits_entry("edlibB200FindRecordHits", true, !out, queries, queryLengths, numQueries, nullptr, 0, &ra,
-                           config, bothStrands, maxHitsPerQuery, &o->aln, &o->records);
+                           nullptr, config, bothStrands, maxHitsPerQuery, &o->aln, &o->records);
+}
+
+EDLIB_API int edlibB200FindPairHits(const char* const* queries, const int* queryLengths, const char* const* targets,
+                                    const int* targetLengths, int numPairs, const EdlibAlignConfig config, int bothStrands,
+                                    long long maxHitsPerPair, EdlibB200HitAlignments* out) {
+    EdlibB200HitAlignments scratch;
+    const PairArgs pa{targets, targetLengths};
+    return find_hits_entry("edlibB200FindPairHits", true, !out, queries, queryLengths, numPairs, nullptr, 0, nullptr, &pa,
+                           config, bothStrands, maxHitsPerPair, out ? out : &scratch, nullptr);
 }
 
 EDLIB_API void edlibB200FreeRecordHits(EdlibB200RecordHits* out) {

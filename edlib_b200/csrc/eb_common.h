@@ -408,6 +408,24 @@ struct HitPlaceParams {
     long long* at;           // hits_place: [job] -> HitParams::at
     int* room;               // hits_place: [job] -> HitParams::room
 };
+// Hits of the per-pair route (edlibB200FindPairHits): one job per (pair, chunk) of the pair's OWN target, swept as a
+// K1 chunk (restart at hs, columns [cs, ce) owned and reported; eb_core.h: lane_hits_job).  The jobs of a pair are
+// consecutive and in column order; HitPlaceParams::plan gives each slot its range (state SEED_WINDOWS).
+struct LaneHitJob {
+    uint64_t qOff;     // into qcodes
+    uint64_t tOff;     // into tcodes: the symbol of target column hs
+    int m;
+    int hs, cs, ce;    // target columns: first swept, first owned, one past the last owned
+};
+struct LaneHitParams {
+    const LaneHitJob* jobs;
+    int numJobs;
+    int k;                   // fixed threshold
+    const uint8_t* qcodes;
+    const uint8_t* tcodes;
+    int ncodes;
+    const uint8_t* eqtab;
+};
 // Start locations and edit scripts of stored hits (edlibB200FindHitAlignments), one slice of stored hits at a time:
 // the lane kernel runs one reversed SHW sweep (start) and one matrix-storing NW sweep + traceback (script) per hit of
 // word class nw; `stage` selects the per-item function of hit_res_kernel.  Hit h of the slice is stored hit
@@ -430,6 +448,7 @@ struct HitResParams {
     const int* qlen;         // [pair]
     const uint64_t* qoff;    // [pair]
     uint64_t tOff;           // offset of the shared target in the packed buffer
+    const uint64_t* tOffPair;  // [pair] offset of the pair's own target (edlibB200FindPairHits), or nullptr: tOff
     const int* cols;         // [stored hit] end column
     const int* scores;       // [stored hit] D(column)
     int* cnt;                // [hits + 1] flags, then their exclusive prefix sums: job of hit h is cnt[h]

@@ -851,6 +851,23 @@ EB_HD void k1_hits_thread(const K1Params& p, const HitParams& h, int slot, int c
     hit_sink_close(h, job, sink);
 }
 
+// Hits of one (pair, chunk) job of the per-pair route (eb_common.h: LaneHitParams): the sweep of k1_hits_thread over
+// the pair's own target, threshold p.k.  hs lies at least 2m columns before cs (or at column 0), so every score of the
+// owned columns is exact.
+template <int NW, class Acc>
+EB_HD void lane_hits_job(const LaneHitParams& p, const HitParams& h, int job, Acc& acc) {
+    HitSink sink;
+    if (!hit_sink_open(h, job, sink)) return;
+    const LaneHitJob J = p.jobs[job];
+    k1_build_peq<NW>(acc, p.qcodes + J.qOff, J.m, MODE_HW, p.ncodes, p.eqtab);
+    K1State<NW> st;
+    k1_init<NW>(st, J.m, p.k);
+    const uint8_t* t = p.tcodes + J.tOff;
+    k1_columns<NW, false, false>(st, acc, PtrSyms{t}, J.cs - J.hs, J.hs, &sink, job, nullptr, nullptr, 0);
+    k1_columns<NW, false, true>(st, acc, PtrSyms{t + (J.cs - J.hs)}, J.ce - J.cs, J.cs, &sink, job, nullptr, nullptr, 0);
+    hit_sink_close(h, job, sink);
+}
+
 // Job j of read `slot` of a hits launch (eb_common.h: HitPlaceParams), j = 0 .. hit_jobs(p, slot) - 1, in column order.
 EB_HD int hit_jobs(const HitPlaceParams& p, int slot) {
     if (!p.plan) return p.chunks;
@@ -1573,7 +1590,7 @@ EB_HD void hit_res_item(const HitResParams& p, int i) {
             const int c = p.cols[slot], s = p.scores[slot], m = p.qlen[pair];
             LJob J;
             J.qOff = p.qoff[pair];
-            J.tOff = p.tOff + (uint64_t)c;  // first symbol read, walking backwards
+            J.tOff = (p.tOffPair ? p.tOffPair[pair] : p.tOff) + (uint64_t)c;  // first symbol read, walking backwards
             J.matOff = 0;
             J.m = m;
             const long long span = (long long)m + s;  // a start further back costs more than s
@@ -1601,7 +1618,7 @@ EB_HD void hit_res_item(const HitResParams& p, int i) {
             const int st = p.starts[i];
             LJob J;
             J.qOff = p.qoff[pair];
-            J.tOff = p.tOff + (uint64_t)st;
+            J.tOff = (p.tOffPair ? p.tOffPair[pair] : p.tOff) + (uint64_t)st;
             J.matOff = (uint64_t)(j / 32) * 32u * p.matStride + (uint64_t)(j % 32);  // interleaved by 32 jobs (LParams::matStep)
             J.m = p.qlen[pair];
             J.n = p.cols[slot] - st + 1;

@@ -106,6 +106,7 @@ EngineTunables::EngineTunables() {
     longSeedMaxK = env_int("EDLIB_B200_LONG_SEED_MAX_K", longSeedMaxK);
     devSliceReads = std::max(64, env_int("EDLIB_B200_SLICE_READS", devSliceReads));
     streamMinPairs = env_int("EDLIB_B200_STREAM_MIN_PAIRS", streamMinPairs);
+    hitRunReads = std::max(1, env_int("EDLIB_B200_HIT_RUN_READS", hitRunReads));
     const int sliceMb = env_int("EDLIB_B200_SLICE_MB", 0);
     if (sliceMb > 0) sliceBytes = (size_t)sliceMb << 20;
     if (sliceMb > 0) pathSliceBytes = (size_t)sliceMb << 20;

@@ -89,6 +89,8 @@ struct Backend {
     // and the per-read totals / placement between the two passes.  A backend without these kernels refuses the call.
     virtual void launch_k1w_hits(const K1WParams&, const HitParams&, int /*nw32*/) { no_kernel("k1w_hits"); }
     virtual void launch_k1_hits(const K1Params&, const HitParams&, int /*nw32*/) { no_kernel("k1_hits"); }
+    // count or fill pass of the per-pair route (edlibB200FindPairHits): (pair, chunk) jobs over each pair's own target
+    virtual void launch_lane_hits(const LaneHitParams&, const HitParams&, int /*nw32*/) { no_kernel("lane_hits"); }
     virtual void launch_hits_total(const HitPlaceParams&) { no_kernel("hits_total"); }
     virtual void launch_hits_place(const HitPlaceParams&) { no_kernel("hits_place"); }
     // start locations / edit scripts of stored hits (eb_common.h: HitResParams)
@@ -166,6 +168,7 @@ struct EngineTunables {
     int collapseEqualities = 1;   // transitive additional equalities: one code per group of equal bytes, no equality table
     int bandKernel = 1;           // k-banded NW sweeps of long queries on the thread-per-alignment band kernel (0: warp kernel)
     int filterSkipRepeats = 1;    // reads the last seed level found too repetitive skip the prefix stages (plain sweep)
+    int hitRunReads = 1 << 18;    // hits: reads per launch group (bounds the per-job arrays of the whole-target and per-pair sweeps)
     EngineTunables();             // reads EDLIB_B200_* environment overrides (used by tests)
 };
 
@@ -213,7 +216,8 @@ public:
     // false when the batch is not of that shape (nothing done), throws on failure.
     bool align_streamed(const BatchInput& in, EdlibAlignResult* results);
     // edlibB200FindHits / edlibB200FindHitAlignments: every end column within config.k of every query over the one
-    // shared target (in.strands: of its reverse complement too), at most maxHits stored per query; config.task LOC /
+    // shared target (edlibB200FindPairHits: over the pair's own target; in.strands: of its reverse complement too), at
+    // most maxHits stored per query; config.task LOC /
     // PATH adds the start location / edit script of every stored hit.  `out` is filled with malloc'd arrays; on
     // failure nothing stays allocated.  Returns EDLIB_STATUS_OK / EDLIB_STATUS_ERROR.  A record target
     // (in.numRecords > 0, edlibB200FindRecordHits): columns and starts count from the start of each hit's record, and

@@ -742,11 +742,12 @@ struct Pass {
     void dev_leftovers();
 
     // ---- hits (edlibB200FindHits; eb_pass_lane.cpp) ----------------------------------------------------------
-    // Runs instead of the distance pass: every end column scoring <= k of every pair over the batch's one target, into
-    // `out` (malloc'd arrays; the two pairs of a read of a strand batch share its cap, forward first).  A pair takes the
-    // seed windows of the first level whose threshold reaches k, or the whole-target sweep (no such level, saturated
-    // plan, repeats, short target, equality table); both count, place, then fill.  task LOC / PATH: then the start
-    // location / edit script of every stored hit (hit_alignments).
+    // Runs instead of the distance pass: every end column scoring <= k of every pair over its target, into `out`
+    // (malloc'd arrays; the two pairs of a read of a strand batch share its cap, forward first).  The pairs of a target
+    // group of at least k1MinGroup pairs (or of the batch's only target) take the seed windows of the first level whose
+    // threshold reaches k, or the whole-target sweep (no such level, saturated plan, repeats, short target, equality
+    // table); every other pair the per-pair route (chunks of its own target, launch_lane_hits).  All routes count,
+    // place, then fill.  task LOC / PATH: then the start location / edit script of every stored hit (hit_alignments).
     // A record target: columns (and starts) are mapped into their records on the device, their records into *records.
     void hits(long long maxHits, int task, EdlibB200HitAlignments* out, int** records);
     // Start locations (and, task PATH, edit scripts) of the S stored hits in dCols / dScores, whose pairs start at

@@ -373,6 +373,20 @@ __global__ void k1_hits_records_kernel(const K1Params p, const HitParams h) {
     k1_hits_thread<NW, SmemPeqAcc<NW>, RecordHitSink>(p, h, slot, (int)blockIdx.y, acc);
 }
 
+// Hits of the per-pair route (eb_core.h: lane_hits_job): one thread per (pair, chunk) job over the pair's own target,
+// symbols from global memory, the profile in shared memory as for lane_kernel.
+template <int NW>
+__global__ void lane_hits_kernel(const LaneHitParams p, const HitParams h) {
+    extern __shared__ __align__(128) unsigned char smem[];
+    const int job = blockIdx.x * blockDim.x + threadIdx.x;
+    if (job >= p.numJobs) return;
+    SmemPeqAcc<NW> acc;
+    acc.codeStride = (uint32_t)blockDim.x * (16u + 4u * SmemPeqAcc<NW>::NWB);
+    acc.a0 = smem_u32(smem) + 16u * threadIdx.x;
+    acc.b0 = smem_u32(smem) + 16u * blockDim.x + 4u * SmemPeqAcc<NW>::NWB * threadIdx.x;
+    lane_hits_job<NW>(p, h, job, acc);
+}
+
 __global__ void hits_total_kernel(const HitPlaceParams p) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < p.numReads) hits_total_item(p, i);
@@ -1039,6 +1053,15 @@ struct CudaBackend : Backend {
             if (h.sepCodes) launch("k1_hits_records", k1_hits_records_kernel<decltype(w)::value>, grid, block, smem, p, h);
             else launch("k1_hits", k1_hits_kernel<decltype(w)::value>, grid, block, smem, p, h);
         });
+    }
+    void launch_lane_hits(const LaneHitParams& p, const HitParams& h, int nw) override {
+        if (p.numJobs <= 0) return;
+        int block = 128;
+        const size_t perThread = (size_t)p.ncodes * (16 + 4 * (nw > 4 ? nw - 4 : 0));
+        while (block > 32 && perThread * block > 96 * 1024) block >>= 1;
+        const size_t smem = perThread * block;
+        if (smem > (size_t)maxSmemOptin) throw std::runtime_error("lane_hits: alphabet too large for shared memory");
+        with_nw(nw, [&](auto w) { launch("lane_hits", lane_hits_kernel<decltype(w)::value>, (p.numJobs + block - 1) / block, block, smem, p, h); });
     }
     void launch_hits_total(const HitPlaceParams& p) override {
         if (p.numReads > 0) launch("hits_total", hits_total_kernel, (p.numReads + 255) / 256, 256, 0, p);

@@ -941,151 +941,242 @@ void Pass::dev_leftovers() {
 // Hits (edlibB200FindHits): every end column within k instead of the minimum.  The seed levels are exact pigeonhole
 // filters: planned with threshold k, the tracked columns of a read's windows cover every end column of every alignment
 // within k, hold every such score exactly and are disjoint and in column order; the whole-target sweep restarts each
-// chunk 2m columns early and reports the columns the chunk owns.  Either way a read's hits are those of its jobs in
-// job order, so no sort is needed: count per job, total per read, the read's place in the output (host), the place of
-// each job, and a fill pass over the jobs that store something.
+// chunk 2m columns early and reports the columns the chunk owns, and so do the (pair, chunk) jobs of the per-pair route
+// over each pair's own target.  Either way a read's hits are those of its jobs in job order, so no sort is needed: count
+// per job, total per read, the read's place in the output (host), the place of each job, and a fill pass over the jobs
+// that store something.
 // =============================================================================================
 namespace {
 // One launch group of the hits pass: reads of one word class on one route, with what the fill pass needs again.
 struct HitRun {
-    int nw = 0, level = -1;  // seed level, or -1: whole-target sweep
+    int t = 0, nw = 0, level = -1;  // target (group routes); seed level, -1: whole-target sweep, -2: per-pair route
     std::vector<int> pairs;
     DevBuf<int> dList, dCount, dRoom, dWinCount;
     DevBuf<long long> dAt;
-    DevBuf<SeedPlan> dPlan;  // seed route
-    WinJobs jobs;            // seed route
-    DevBuf<int> dK;          // whole-target sweep: k per read
+    DevBuf<SeedPlan> dPlan;      // seed route: the windows of each read; per-pair route: the jobs of each read
+    WinJobs jobs;                // seed route
+    DevBuf<int> dK;              // whole-target sweep: k per read
+    DevBuf<LaneHitJob> dJobs;    // per-pair route
     int numJobs = 0, chunks = 0, chunkLen = 0;
 };
-constexpr int HIT_RUN_READS = 1 << 18;  // reads per launch group (bounds the per-job arrays of a whole-target sweep)
+constexpr int HIT_RUN_JOBS = 1 << 22;  // jobs per launch group of the per-pair route (at most 4096 per read)
 }  // namespace
 
 void Pass::hits(long long maxHits, int task, EdlibB200HitAlignments* outAln, int** records) {
     EdlibB200Hits* out = &outAln->hits;
-    if (p->tg.size() != 1) throw std::runtime_error("internal: hits need one shared target");
-    const Target& tg = p->tg[0];
-    const int n = tg.len;
-    // several records: the sweeps run over all of them at once, and a separator column is never a hit
-    const uint8_t* sepCodes = p->sep >= 0 ? p->dSeq.p + tg.off : nullptr;
+    const int T = (int)p->tg.size();
+    // several records (the batch's one target): the sweeps run over all of them at once, and a separator column is
+    // never a hit
+    const uint8_t* sepCodes = p->sep >= 0 ? p->dSeq.p + p->tg[0].off : nullptr;
     const int Q = p->strands ? N / 2 : N;
-    // ---- routes: the first seed level whose threshold reaches k itself, else the whole-target sweep ----
-    const bool seeds = n >= tun.filterMinTarget && !p->hasEq && tun.filterSeedK > 0 && tun.filterSeedLevels > 0 && seed_index(0);
-    std::vector<std::unique_ptr<HitRun>> runs;
-    std::vector<int> full[9];
-    {
-        std::map<std::pair<int, int>, std::vector<int>> groups;  // (level, nw) -> pairs
-        for (int pair = 0; pair < N; ++pair) {
-            const int m = p->qlen[pair], nw = ceil_div(m, 32);
-            int level = -1;
-            for (int l = 0; seeds && l < tun.filterSeedLevels && level < 0; ++l)
-                if (seedIdx->Ls[l] > 0 && seed_threshold(m, k, seedIdx->Ls[l], tun.filterSeedK, -1) == k) level = l;
-            if (level < 0) full[nw].push_back(pair);
-            else groups[std::make_pair(level, nw)].push_back(pair);
+    // ---- routes per target group: a group of k1MinGroup pairs (or the batch's only target) takes the seed or
+    // whole-target routes over its target, every other pair the per-pair route; a pair with an empty target has no hits
+    std::vector<std::vector<int>> byTarget((size_t)T);
+    for (int pair = 0; pair < N; ++pair)
+        if (p->tlen[pair] > 0) byTarget[(size_t)p->tidx[pair]].push_back(pair);
+    std::vector<int> groupTargets, perPair[9];
+    for (int t = 0; t < T; ++t) {
+        const std::vector<int>& list = byTarget[(size_t)t];
+        if (T == 1 || (int)list.size() >= tun.k1MinGroup) {
+            if (!list.empty()) groupTargets.push_back(t);
+        } else {
+            for (int pair : list) perPair[ceil_div(p->qlen[pair], 32)].push_back(pair);
         }
-        for (auto& kv : groups)
-            for (size_t a = 0; a < kv.second.size(); a += HIT_RUN_READS) {
-                runs.emplace_back(new HitRun());
-                HitRun& r = *runs.back();
-                r.level = kv.first.first;
-                r.nw = kv.first.second;
-                r.pairs.assign(kv.second.begin() + a, kv.second.begin() + std::min(kv.second.size(), a + HIT_RUN_READS));
-            }
     }
+    std::vector<std::unique_ptr<HitRun>> runs;
     DevBuf<long long> dPairCount(be, (size_t)N);
     be->zero(dPairCount.p, (size_t)N * sizeof(long long));
-    // ---- count pass of the seed route: plan at threshold k (one host wait for the window count, one for the plans) ----
-    for (auto& rp : runs) {
-        HitRun& r = *rp;
-        const int g = (int)r.pairs.size();
-        r.dList.alloc(be, g);
-        r.dList.upload(r.pairs.data(), g);
-        const std::vector<int> thr((size_t)g, k);
-        DevBuf<int> dThr(be, g);
-        dThr.upload(thr.data(), g);
-        r.dPlan.alloc(be, g);
-        r.dWinCount.alloc(be, 1);
-        be->zero(r.dWinCount.p, sizeof(int));
-        SeedPlanParams sp = seed_plan_params(tg, r.level);
-        sp.readList = r.dList.p;
-        sp.thr = dThr.p;
-        sp.numReads = g;
-        sp.maxLen = 32 * r.nw;
-        sp.plan = r.dPlan.p;
-        r.jobs.count = r.dWinCount.p;
-        const int perRead = r.level == 0 ? 8 : r.level == 1 ? 96 : r.level == 2 ? 400 : 1500;
-        r.numJobs = plan_windows(sp, r.jobs, (int)std::min<long long>((long long)g * perRead + 4096, 1LL << 28), true);
-        std::vector<SeedPlan> plan((size_t)g);
-        be->d2h(plan.data(), r.dPlan.p, (size_t)g * sizeof(SeedPlan));
-        stats.d2hBytes += (long long)g * (long long)sizeof(SeedPlan);
-        stats.filterWindows += r.numJobs;
-        for (int s = 0; s < g; ++s) {
-            // saturated: more candidates than the level holds, seeds of repeats, or no room in the job arrays
-            if (plan[(size_t)s].state == SEED_SATURATED) full[r.nw].push_back(r.pairs[(size_t)s]);
-            else stats.filterDecided++;
-        }
-        r.dCount.alloc(be, (size_t)std::max(r.numJobs, 1));
-        if (r.numJobs > 0) {
-            const HitParams h{r.dCount.p, nullptr, nullptr, nullptr, nullptr, sepCodes, p->sep};
-            be->launch_k1w_hits(window_params(tg, r.jobs, r.numJobs), h, r.nw);
-        }
-        HitPlaceParams hp;
-        memset(&hp, 0, sizeof(hp));
-        hp.plan = r.dPlan.p;
-        hp.numReads = g;
-        hp.readList = r.dList.p;
-        hp.count = r.dCount.p;
-        hp.pairCount = dPairCount.p;
-        be->launch_hits_total(hp);
-    }
-    trace.mark("hits: seed windows counted");
-    // ---- count pass of the whole-target sweep (launched after the seed route: it overwrites the totals of saturated reads) ----
     K1Params kp;
     memset(&kp, 0, sizeof(kp));
-    kp.tcodes = p->dSeq.p + tg.off;
-    kp.n = n;
     kp.qcodes = p->dSeq.p;
     kp.qoff = p->dQoff.p;
     kp.qlen = p->dQlen.p;
     kp.mode = MODE_HW;
     kp.ncodes = p->ncodes;
     kp.eqtab = p->hasEq ? p->dEqtab.p : nullptr;
-    const size_t seedRuns = runs.size();
-    for (int nw = 1; nw <= 8; ++nw)
-        for (size_t a = 0; a < full[nw].size(); a += HIT_RUN_READS) {
-            runs.emplace_back(new HitRun());
-            HitRun& r = *runs.back();
-            r.nw = nw;
-            r.pairs.assign(full[nw].begin() + a, full[nw].begin() + std::min(full[nw].size(), a + HIT_RUN_READS));
+    for (int t : groupTargets) {
+        const Target& tg = p->tg[(size_t)t];
+        const int n = tg.len;
+        // ---- routes: the first seed level whose threshold reaches k itself, else the whole-target sweep ----
+        const bool seeds = n >= tun.filterMinTarget && !p->hasEq && tun.filterSeedK > 0 && tun.filterSeedLevels > 0 && seed_index(t);
+        const size_t firstRun = runs.size();
+        std::vector<int> full[9];
+        {
+            std::map<std::pair<int, int>, std::vector<int>> groups;  // (level, nw) -> pairs
+            for (int pair : byTarget[(size_t)t]) {
+                const int m = p->qlen[pair], nw = ceil_div(m, 32);
+                int level = -1;
+                for (int l = 0; seeds && l < tun.filterSeedLevels && level < 0; ++l)
+                    if (seedIdx->Ls[l] > 0 && seed_threshold(m, k, seedIdx->Ls[l], tun.filterSeedK, -1) == k) level = l;
+                if (level < 0) full[nw].push_back(pair);
+                else groups[std::make_pair(level, nw)].push_back(pair);
+            }
+            for (auto& kv : groups)
+                for (size_t a = 0; a < kv.second.size(); a += (size_t)tun.hitRunReads) {
+                    runs.emplace_back(new HitRun());
+                    HitRun& r = *runs.back();
+                    r.t = t;
+                    r.level = kv.first.first;
+                    r.nw = kv.first.second;
+                    r.pairs.assign(kv.second.begin() + a, kv.second.begin() + std::min(kv.second.size(), a + (size_t)tun.hitRunReads));
+                }
+        }
+        // ---- count pass of the seed route: plan at threshold k (one host wait for the window count, one for the plans) ----
+        const size_t seedEnd = runs.size();
+        for (size_t ri = firstRun; ri < seedEnd; ++ri) {
+            HitRun& r = *runs[ri];
             const int g = (int)r.pairs.size();
-            stats.filterFallback += g;
-            const LaneGroup c{0, nw, r.pairs, tg, n, {}, {}, {}, {}};
-            lane_geometry(c, g, nw, r.chunks, r.chunkLen, true);
-            r.numJobs = r.chunks * g;
             r.dList.alloc(be, g);
             r.dList.upload(r.pairs.data(), g);
-            const std::vector<int> kk((size_t)g, k);
-            r.dK.alloc(be, g);
-            r.dK.upload(kk.data(), g);
-            r.dCount.alloc(be, (size_t)r.numJobs);
-            kp.readList = r.dList.p;
-            kp.kInit = r.dK.p;
-            kp.numReads = g;
-            kp.chunks = r.chunks;
-            kp.chunkLen = r.chunkLen;
-            kp.halo = 64 * nw;
-            const HitParams h{r.dCount.p, nullptr, nullptr, nullptr, nullptr, sepCodes, p->sep};
-            be->launch_k1_hits(kp, h, nw);
-            stats.k1Cells += (long long)g * 32 * nw * (long long)n;
+            const std::vector<int> thr((size_t)g, k);
+            DevBuf<int> dThr(be, g);
+            dThr.upload(thr.data(), g);
+            r.dPlan.alloc(be, g);
+            r.dWinCount.alloc(be, 1);
+            be->zero(r.dWinCount.p, sizeof(int));
+            SeedPlanParams sp = seed_plan_params(tg, r.level);
+            sp.readList = r.dList.p;
+            sp.thr = dThr.p;
+            sp.numReads = g;
+            sp.maxLen = 32 * r.nw;
+            sp.plan = r.dPlan.p;
+            r.jobs.count = r.dWinCount.p;
+            const int perRead = r.level == 0 ? 8 : r.level == 1 ? 96 : r.level == 2 ? 400 : 1500;
+            r.numJobs = plan_windows(sp, r.jobs, (int)std::min<long long>((long long)g * perRead + 4096, 1LL << 28), true);
+            std::vector<SeedPlan> plan((size_t)g);
+            be->d2h(plan.data(), r.dPlan.p, (size_t)g * sizeof(SeedPlan));
+            stats.d2hBytes += (long long)g * (long long)sizeof(SeedPlan);
+            stats.filterWindows += r.numJobs;
+            for (int s = 0; s < g; ++s) {
+                // saturated: more candidates than the level holds, seeds of repeats, or no room in the job arrays
+                if (plan[(size_t)s].state == SEED_SATURATED) full[r.nw].push_back(r.pairs[(size_t)s]);
+                else stats.filterDecided++;
+            }
+            r.dCount.alloc(be, (size_t)std::max(r.numJobs, 1));
+            if (r.numJobs > 0) {
+                const HitParams h{r.dCount.p, nullptr, nullptr, nullptr, nullptr, sepCodes, p->sep};
+                be->launch_k1w_hits(window_params(tg, r.jobs, r.numJobs), h, r.nw);
+            }
             HitPlaceParams hp;
             memset(&hp, 0, sizeof(hp));
-            hp.chunks = r.chunks;
+            hp.plan = r.dPlan.p;
             hp.numReads = g;
             hp.readList = r.dList.p;
             hp.count = r.dCount.p;
             hp.pairCount = dPairCount.p;
             be->launch_hits_total(hp);
         }
-    trace.mark("hits: whole-target sweeps counted");
+        trace.mark("hits: seed windows counted");
+        // ---- count pass of the whole-target sweep (launched after the seed route: it overwrites the totals of saturated reads) ----
+        kp.tcodes = p->dSeq.p + tg.off;
+        kp.n = n;
+        for (int nw = 1; nw <= 8; ++nw)
+            for (size_t a = 0; a < full[nw].size(); a += (size_t)tun.hitRunReads) {
+                runs.emplace_back(new HitRun());
+                HitRun& r = *runs.back();
+                r.t = t;
+                r.nw = nw;
+                r.pairs.assign(full[nw].begin() + a, full[nw].begin() + std::min(full[nw].size(), a + (size_t)tun.hitRunReads));
+                const int g = (int)r.pairs.size();
+                stats.filterFallback += g;
+                const LaneGroup c{t, nw, r.pairs, tg, n, {}, {}, {}, {}};
+                lane_geometry(c, g, nw, r.chunks, r.chunkLen, true);
+                r.numJobs = r.chunks * g;
+                r.dList.alloc(be, g);
+                r.dList.upload(r.pairs.data(), g);
+                const std::vector<int> kk((size_t)g, k);
+                r.dK.alloc(be, g);
+                r.dK.upload(kk.data(), g);
+                r.dCount.alloc(be, (size_t)r.numJobs);
+                kp.readList = r.dList.p;
+                kp.kInit = r.dK.p;
+                kp.numReads = g;
+                kp.chunks = r.chunks;
+                kp.chunkLen = r.chunkLen;
+                kp.halo = 64 * nw;
+                const HitParams h{r.dCount.p, nullptr, nullptr, nullptr, nullptr, sepCodes, p->sep};
+                be->launch_k1_hits(kp, h, nw);
+                stats.k1Cells += (long long)g * 32 * nw * (long long)n;
+                HitPlaceParams hp;
+                memset(&hp, 0, sizeof(hp));
+                hp.chunks = r.chunks;
+                hp.numReads = g;
+                hp.readList = r.dList.p;
+                hp.count = r.dCount.p;
+                hp.pairCount = dPairCount.p;
+                be->launch_hits_total(hp);
+            }
+        trace.mark("hits: whole-target sweeps counted");
+    }
+    // ---- count pass of the per-pair route: (pair, chunk) jobs over each pair's own target, a pair's jobs consecutive
+    // and in column order, chunk lengths as lane_geometry cuts a target for the route's pairs of the word class ----
+    for (int nw = 1; nw <= 8; ++nw) {
+        const std::vector<int>& pl = perPair[nw];
+        if (pl.empty()) continue;
+        const int G = (int)pl.size();
+        stats.filterFallback += G;
+        int blockThreads = 0, residentCtas = 0;
+        be->k1_shape(nw, p->ncodes, G, &blockThreads, &residentCtas);
+        std::vector<int> chunks((size_t)G), chunkLen((size_t)G);
+        for (int i = 0; i < G; ++i) {
+            const int t = p->tidx[pl[(size_t)i]];
+            const Target& tg = p->tg[(size_t)t];
+            if (residentCtas > 0) {
+                const LaneGroup c{t, nw, pl, tg, tg.len, {}, {}, {}, {}};
+                lane_geometry(c, G, nw, chunks[(size_t)i], chunkLen[(size_t)i], true);
+            } else {  // no K1 shape for this alphabet (launch_lane_hits decides whether the jobs run): one chunk
+                chunks[(size_t)i] = 1;
+                chunkLen[(size_t)i] = tg.len;
+            }
+        }
+        for (int a = 0; a < G;) {
+            int b = a, numJobs = 0;
+            while (b < G && b - a < tun.hitRunReads && numJobs + chunks[(size_t)b] <= HIT_RUN_JOBS) numJobs += chunks[(size_t)b++];
+            runs.emplace_back(new HitRun());
+            HitRun& r = *runs.back();
+            r.nw = nw;
+            r.level = -2;
+            r.pairs.assign(pl.begin() + a, pl.begin() + b);
+            r.numJobs = numJobs;
+            const int g = b - a;
+            std::vector<SeedPlan> plan((size_t)g);
+            std::vector<LaneHitJob> jobs;
+            jobs.reserve((size_t)numJobs);
+            for (int s = 0; s < g; ++s) {
+                const int pair = r.pairs[(size_t)s], m = p->qlen[pair];
+                const Target& tg = p->tg[(size_t)p->tidx[pair]];
+                const int C = chunks[(size_t)(a + s)], L = chunkLen[(size_t)(a + s)];
+                plan[(size_t)s] = SeedPlan{(int)jobs.size(), C, SEED_WINDOWS, k};
+                for (int c = 0; c < C; ++c) {
+                    const int cs = (int)std::min<long long>((long long)c * L, tg.len);
+                    const int ce = (int)std::min<long long>((long long)cs + L, tg.len);
+                    const int hs = std::max(0, cs - 64 * nw);  // >= 2m columns of restart: the owned scores are exact
+                    jobs.push_back(LaneHitJob{p->qoff[pair], tg.off + (uint64_t)hs, m, hs, cs, ce});
+                }
+                stats.k1Cells += 32LL * nw * tg.len;
+            }
+            a = b;
+            r.dList.alloc(be, g);
+            r.dList.upload(r.pairs.data(), g);
+            r.dPlan.alloc(be, g);
+            r.dPlan.upload(plan.data(), g);
+            r.dJobs.alloc(be, (size_t)numJobs);
+            r.dJobs.upload(jobs.data(), (size_t)numJobs);
+            r.dCount.alloc(be, (size_t)numJobs);
+            const LaneHitParams lp{r.dJobs.p, numJobs, k, p->dSeq.p, p->dSeq.p, p->ncodes, p->hasEq ? p->dEqtab.p : nullptr};
+            const HitParams h{r.dCount.p, nullptr, nullptr, nullptr, nullptr, nullptr, -1};
+            be->launch_lane_hits(lp, h, nw);
+            HitPlaceParams hp;
+            memset(&hp, 0, sizeof(hp));
+            hp.plan = r.dPlan.p;
+            hp.numReads = g;
+            hp.readList = r.dList.p;
+            hp.count = r.dCount.p;
+            hp.pairCount = dPairCount.p;
+            be->launch_hits_total(hp);
+        }
+    }
+    trace.mark("hits: per-pair sweeps counted");
     // ---- the place of every read in the output: counts per query, the first maxHits stored, forward strand first ----
     std::vector<long long> cnt((size_t)N), base((size_t)N), stored((size_t)N);
     be->d2h(cnt.data(), dPairCount.p, (size_t)N * sizeof(long long));
@@ -1140,7 +1231,7 @@ void Pass::hits(long long maxHits, int task, EdlibB200HitAlignments* outAln, int
         r.dRoom.alloc(be, (size_t)r.numJobs);
         HitPlaceParams hp;
         memset(&hp, 0, sizeof(hp));
-        hp.plan = ri < seedRuns ? r.dPlan.p : nullptr;
+        hp.plan = r.level != -1 ? r.dPlan.p : nullptr;
         hp.chunks = r.chunks;
         hp.numReads = g;
         hp.readList = r.dList.p;
@@ -1151,9 +1242,12 @@ void Pass::hits(long long maxHits, int task, EdlibB200HitAlignments* outAln, int
         hp.room = r.dRoom.p;
         be->launch_hits_place(hp);
         const HitParams h{nullptr, r.dAt.p, r.dRoom.p, dCols.p, dScores.p, sepCodes, p->sep};
-        if (ri < seedRuns) {
+        const Target& tg = p->tg[(size_t)r.t];
+        if (r.level >= 0) {
             be->launch_k1w_hits(window_params(tg, r.jobs, r.numJobs), h, r.nw);
-        } else {
+        } else if (r.level == -1) {
+            kp.tcodes = p->dSeq.p + tg.off;
+            kp.n = tg.len;
             kp.readList = r.dList.p;
             kp.kInit = r.dK.p;
             kp.numReads = g;
@@ -1161,6 +1255,9 @@ void Pass::hits(long long maxHits, int task, EdlibB200HitAlignments* outAln, int
             kp.chunkLen = r.chunkLen;
             kp.halo = 64 * r.nw;
             be->launch_k1_hits(kp, h, r.nw);
+        } else {
+            const LaneHitParams lp{r.dJobs.p, r.numJobs, k, p->dSeq.p, p->dSeq.p, p->ncodes, p->hasEq ? p->dEqtab.p : nullptr};
+            be->launch_lane_hits(lp, h, r.nw);
         }
     }
     dScores.download(out->scores, (size_t)S);
@@ -1232,6 +1329,13 @@ void Pass::hit_alignments(int task, long long S, const std::vector<long long>& s
     if (path) H = std::min(H, (long long)(0x7fffffff / maxOps) - 1);  // so do the script lengths
     H = std::min(H, S);
     const uint64_t tOff = p->tg[0].off;
+    DevBuf<uint64_t> dTOffPair;  // pairs over their own targets: the offset of each pair's target
+    if (p->tg.size() > 1) {
+        std::vector<uint64_t> off((size_t)N);
+        for (int pair = 0; pair < N; ++pair) off[(size_t)pair] = p->tg[(size_t)p->tidx[pair]].off;
+        dTOffPair.alloc(be, (size_t)N);
+        dTOffPair.upload(off.data(), (size_t)N);
+    }
     DevBuf<int> dErr(be, 1);
     be->zero(dErr.p, sizeof(int));
     DevBuf<int> dCnt(be, (size_t)H + 1), dStart(be, (size_t)H), dLen(be, path ? (size_t)H + 1 : 1);
@@ -1247,6 +1351,7 @@ void Pass::hit_alignments(int task, long long S, const std::vector<long long>& s
         hp.qlen = p->dQlen.p;
         hp.qoff = p->dQoff.p;
         hp.tOff = tOff;
+        hp.tOffPair = p->tg.size() > 1 ? dTOffPair.p : nullptr;
         hp.cols = dCols;
         hp.scores = dScores;
         hp.cnt = dCnt.p;

@@ -192,6 +192,32 @@ EDLIB_API int edlibB200FindRecordHits(const char* const* queries, const int* que
 /* Frees the arrays of edlibB200FindRecordHits and clears the struct. */
 EDLIB_API void edlibB200FreeRecordHits(EdlibB200RecordHits* out);
 
+/* Every hit of each query in its own target: pair i searches queries[i] in targets[i] only (a read's candidate region,
+ * its amplicon, the locus a guide is assigned to), all pairs in one call.
+ *
+ * For a pair with targetLengths[i] >= 1, everything of entry i (counts[i], the stored hits at [offsets[i],
+ * offsets[i+1]), their columns, scores, strands, starts and scripts) is exactly what edlibB200FindHitAlignments(
+ * &queries[i], &queryLengths[i], 1, targets[i], targetLengths[i], config, bothStrands, maxHitsPerPair, ...) gives for
+ * its one query; columns and starts count from the start of targets[i].  A pair with targetLengths[i] == 0 has no
+ * hits (columns run over 0 <= c < n), and its targets[i] may be NULL.  The cap and the strand order apply per pair.
+ * hits.numQueries = numPairs; edlibB200FreeHitAlignments releases the result.
+ *
+ * Pairs that share a target (the same pointer and length) are one target group: a group of many pairs is searched as
+ * edlibB200FindHitAlignments searches its target, the other pairs by a sweep of each pair over its own target.  A call
+ * whose pairs all share one target runs exactly as edlibB200FindHitAlignments over that target.
+ *
+ * Accepted: numPairs >= 0, and per pair what edlibB200FindHitAlignments accepts: 1 <= queryLengths[i] <= 256,
+ * config.k >= 0, config.mode == EDLIB_MODE_HW, config.task EDLIB_TASK_DISTANCE, EDLIB_TASK_LOC or EDLIB_TASK_PATH, any
+ * additional equalities, maxHitsPerPair >= 0; targetLengths[i] >= 0 with targets[i] non-NULL when targetLengths[i] > 0.
+ * Anything else returns EDLIB_STATUS_ERROR with a message in edlibB200LastError (starting with "edlibB200FindPairHits:"
+ * for invalid input) and *out left empty.  edlibB200LastStats: filterWindows = seed windows planned, filterDecided =
+ * pair-strands whose hits came from seed windows, filterFallback = pair-strands swept over their whole target (a group's
+ * or their own); kernel time and launches include every sweep. */
+EDLIB_API int edlibB200FindPairHits(const char* const* queries, const int* queryLengths,
+                                    const char* const* targets, const int* targetLengths, int numPairs,
+                                    const EdlibAlignConfig config, int bothStrands, long long maxHitsPerPair,
+                                    EdlibB200HitAlignments* out);
+
 /* Each query aligned (HW mode) against a reference of several records in one call, with the result of its best record.
  *
  * For query q let A(r) = edlibAlign(q, records[r], config).  The best record r* is the lowest index among the records
